@@ -1,5 +1,5 @@
 // alva_common.cuh -- shared device helpers (PTX wrappers for mbarrier / TMA, SWAR byte math) and the
-// host-side context for libalva_b200.so.  sm_100a only.
+// host-side context for libalva_b200.so.  sm_90a only.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -12,7 +12,7 @@ struct alva_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;
     bool own_stream = false;
-    int num_sms = 148;
+    int num_sms = 132;
     long long launches = 0;
     // scratch (grown on demand)
     void* scratch = nullptr;

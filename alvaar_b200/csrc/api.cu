@@ -84,8 +84,8 @@ extern "C" alva_ctx* alva_ctx_create(int device, void* stream) {
     if ((e = cudaGetDevice(&curdev)) != cudaSuccess || curdev != device) { alva_set_error("cudaSetDevice(%d): %s", device, cudaGetErrorString(e)); return nullptr; }
     cudaDeviceProp prop;
     if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) { alva_set_error("props: %s", cudaGetErrorString(e)); return nullptr; }
-    if (prop.major != 10) {
-        alva_set_error("alva_ctx_create: device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {
+        alva_set_error("alva_ctx_create: device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major, prop.minor);
         return nullptr;
     }
     alva_ctx* ctx = new alva_ctx();

@@ -1,4 +1,4 @@
-// ba.cu -- local bundle adjustment (anchored inverse depth, SE(3) poses) on sm_100a: residual/Jacobian build,
+// ba.cu -- local bundle adjustment (anchored inverse depth, SE(3) poses) on sm_90a: residual/Jacobian build,
 // Huber re-weighting, Schur-complement reduction to the reduced camera system, dense Cholesky, back-substitution and
 // Ceres' Levenberg-Marquardt trust-region control flow -- all on the device, batched over independent problems.
 //
@@ -795,7 +795,7 @@ __global__ void __launch_bounds__(128) ba_schur_kernel(const BaProblem* __restri
 }
 
 // ------------------------------------------------------------------------------------------ dense Schur term on tensor cores
-// S -= Wt' * Wt  with Wt [K = nlm_pad][128] row-major, FP64 tensor-core MMA (mma.sync.m8n8k4.f64 -> SASS DMMA; tcgen05 has
+// S -= Wt' * Wt  with Wt [K = nlm_pad][128] row-major, FP64 tensor-core MMA (mma.sync.m8n8k4.f64 -> SASS DMMA; wgmma has
 // no FP64 kind).  Grid: (16 output blocks of 32x32) x (K splits) x problems; 4 warps per CTA interleave the K steps, the
 // four partial 32x32 blocks are summed in shared memory and added to S with one FP64 atomic per element.
 __device__ __forceinline__ void dmma_m8n8k4(double& c0, double& c1, double a, double b) {
@@ -965,7 +965,7 @@ __device__ __forceinline__ void gather_entry(const BaProblem& P, uint64_t en, co
 // keeps a private 6x6 (+ rhs) accumulator, then a fixed-order shuffle + shared-memory reduction.  Diagonal parts leave their
 // partial sums in a scratch slot; the part that arrives last (ticket) adds the GA_SPLIT slots in slot order.  The block and its
 // mirror are stored -- no floating-point atomics, bit-reproducible.
-constexpr int GA_THREADS = 64, GA_SPLIT = 8;   // (one warp per part x 16 parts measured the same: 0.91 vs 0.92 ms per batch)
+constexpr int GA_THREADS = 64, GA_SPLIT = 8;   // 2 warps per part x 8 parts (the combine loop is valid for any CTA size)
 constexpr int GA_GRID = NBMAX * GA_SPLIT + (MAXKEYS - NBMAX);   // diagonal parts first, then the strictly upper blocks
 __global__ void __launch_bounds__(GA_THREADS, 8) ba_gather_kernel(const BaProblem* __restrict__ probs, BaDims D) {
     const BaProblem P = probs[blockIdx.y];
@@ -1051,8 +1051,8 @@ __global__ void __launch_bounds__(GA_THREADS, 8) ba_gather_kernel(const BaProble
 // matrix is cut into 4 x 4 tiles, one per thread (528 tiles, column-block-major, so whole warps retire as the elimination moves
 // right); V = L D is built in place.  Per column j: the threads holding it publish the column through shared memory (double
 // buffered: ONE barrier per column), then every live tile takes its rank-1 update  a[i][c] -= V[i][j] (V[c][j] / d_j)  from 8
-// shared-memory words -- 16 FP64 FMAs against 8 loads, where the left-looking form spent three loads per multiply-add and was
-// shared-memory-bandwidth bound (113 us; profiles/r02_kernels_full.txt).  Row n of the matrix is the right-hand side, so the
+// shared-memory words -- 16 FP64 FMAs against 8 loads, where a left-looking form spends three loads per multiply-add and is
+// shared-memory-bandwidth bound.  Row n of the matrix is the right-hand side, so the
 // forward substitution z = L^-1 b falls out of the same updates.  Then x = L^-T D^-1 z by warp 0 (lane-strided, registers).
 // No square roots; fixed operation order (bit-reproducible).  yf = S^-1 rhs.
 constexpr int CH_TILES = 32 * 33 / 2, CH_THREADS = (CH_TILES + 31) / 32 * 32;   // 528 tiles -> 544 threads

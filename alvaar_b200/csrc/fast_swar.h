@@ -6,8 +6,7 @@
 // IMAD.HI packing, as before); the 8 antipodal flag words are assembled from them: a byte permute across the neighbouring lane's
 // packed word for the column shift (one SHFL + one PRMT) and a per-byte bit shift for the row shift.  A warp holds 8 rows, so
 // the first dy rows of an antipodal element have their source outside the warp's rows and are still computed directly (15 of 64
-// element-rows).  Per thread: 8 x 8 + 15 = 79 element-rows instead of 128, + 8 x ~4 assembly instructions: about a third off the
-// pre-test, which is a third of the kernel (profiles/r01f_frontend_full.txt).
+// element-rows).  Per thread: 8 x 8 + 15 = 79 element-rows instead of 128, + 8 x ~4 assembly instructions.
 //
 // Layout (as frontend.cu): a lane owns one 32-bit word = 4 horizontally adjacent pixels, over 8 consecutive rows; result / flag
 // words carry bit 8 j + i for pixel j (byte), row i.  Ring numbering (OpenCV's): 0 (0,+3) 1 (+1,+3) 2 (+2,+2) 3 (+3,+1) 4 (+3,0)

@@ -1,4 +1,4 @@
-// frontend.cu -- RGBA->gray, Gaussian pyramid and FAST-9 (+score, +3x3 NMS) for sm_100a.
+// frontend.cu -- RGBA->gray, Gaussian pyramid and FAST-9 (+score, +3x3 NMS) for sm_90a.
 //
 // What is computed (bit-exact with the reference; the CPU restatement is oracle/alva_oracle.c):
 //   gray   : cv::cvtColor(RGBA2GRAY)           reference call site src/slam/src/system.cpp:111-112
@@ -6,7 +6,7 @@
 //                                              video/src/lkpyramid.cpp:726-822, imgproc/src/pyramids.cpp:783-900
 //   FAST   : cv::FAST(thr, nms, TYPE_9_16)     opencv features2d/src/fast.cpp:57-292, fast_score.cpp:119-210
 //
-// How (B200-first, HBM-bound integer/byte work -- no tensor cores here):
+// How (HBM-bound integer/byte work -- no tensor cores here):
 //   * one CTA per 120x62 pixel tile; the RGBA box (128x70 px, 35 KB) arrives by ONE TMA bulk-tensor
 //     copy (cp.async.bulk.tensor.3d, zero-filled out of bounds) signalled on an mbarrier;
 //   * gray is produced once into shared memory (4 px / thread, 128-bit LDS, 32-bit STS) and streamed
@@ -276,7 +276,7 @@ frontend_tile_kernel(const __grid_constant__ CUtensorMap tmap, const FrontendPar
         if (ANTI && w4) {
             // experimental instantiation: the same conversion and stores with the row / width tests hoisted out of the rounds
             // (the default loop below re-tests w % 4 and carries the byte-store fallback in every round: more predicate and
-            // branch scaffolding than arithmetic, profiles/r01f_frontend_full.txt)
+            // branch scaffolding than arithmetic)
             const int by_end = min(4 + TH, h - y0 + 4);   // box rows [4, by_end) are image rows of this tile
 #pragma unroll
             for (int it = 0; it < ROUNDS; it++) {
@@ -493,12 +493,12 @@ frontend_tile_kernel(const __grid_constant__ CUtensorMap tmap, const FrontendPar
 }
 
 // ======================================================================================== variant 2
-// Same tile geometry, same results; what changed against frontend_tile_kernel (profiles/r01f_frontend_full.txt named the costs):
-//   * gray: row / width tests hoisted out of the rounds (the conversion was 18 % IDP and 80 % scaffolding);
+// Same tile geometry, same results; what changed against frontend_tile_kernel:
+//   * gray: row / width tests hoisted out of the rounds (the conversion is little arithmetic and much scaffolding);
 //   * pyramid L1: a thread owns 4 adjacent outputs x 2 rows (7 gray rows x {LDS.32, LDS.64, LDS.32}) instead of 2 x 4;
 //   * FAST pre-test with antipodal flag sharing (fast_swar.h);
 //   * candidate compaction on the TRANSPOSED bit matrix: a lane's 4 x 8 pixel block is either empty or crowded (corner
-//     clusters), so the per-lane emit loop ran at 14.6 active lanes; after a 32 x 32 bit transpose across the warp (2 PRMT + 3
+//     clusters), so the per-lane emit loop runs with few active lanes; after a 32 x 32 bit transpose across the warp (2 PRMT + 3
 //     mask stages on SHFL.BFLY) lane b owns bit position b = (pixel j, row i) of all 32 lanes -- pixels 4 apart in one row,
 //     which no cluster fills -- and the loop is balanced.  The queue order that results (same row, distinct words) also makes
 //     the 16 ring loads of the scoring phase almost bank-conflict free;
@@ -506,10 +506,9 @@ frontend_tile_kernel(const __grid_constant__ CUtensorMap tmap, const FrontendPar
 //     ~4 % of the pixels with full lanes instead of re-walking every candidate; the score tile has a 33-word pitch.
 //   * 120 x 60 tiles (720 and 1080 are multiples of 60: no ragged bottom row) and the score tile folded into the idle RGBA
 //     staging buffer: 44.8 KB of shared memory per CTA instead of 54.4 -> 5 CTAs per SM (40 warps) instead of 4.
-//   * (profiles/r02a_frontend_v2_4cta_full.txt, per-line counts) a (tiles_x, tiles_y, frames) grid instead of two run-time
-//     divisions per warp (4.7 % of the instructions); each warp sends its keypoints straight to the frame's list (one global
+//   * a (tiles_x, tiles_y, frames) grid instead of two run-time divisions per warp; each warp sends its keypoints straight to the frame's list (one global
 //     atomic per warp) instead of a tile list + two barriers + a copy loop; the pyramid's edge words come from the neighbour
-//     lanes (the 2-way conflicted 32-bit loads were 23 % of the excess shared-memory wavefronts); 128-bit score clears;
+//     lanes (instead of 2-way bank-conflicted 32-bit loads); 128-bit score clears;
 //     optionally the tile `prefetch` frames ahead is pulled into L2 by TMA.
 constexpr int TH2 = 60, BH2 = TH2 + 8;    // tile interior rows / loaded box rows
 constexpr int SR2 = TH2 + 2;              // score rows: image y0-1 .. y0+TH2

@@ -1,4 +1,4 @@
-// hamming.cu -- brute-force Hamming 2-NN over 256-bit descriptors, sm_100a.
+// hamming.cu -- brute-force Hamming 2-NN over 256-bit descriptors, sm_90a.
 //
 // Reference behaviour (exact): cv::BFMatcher(NORM_HAMMING).knnMatch(k = 2)
 //   opencv features2d/src/matchers.cpp:757 -> core/src/batch_distance.cpp:103-123 (batchDistHamming),

@@ -1,4 +1,4 @@
-// hamming_mma.cu -- brute-force Hamming 2-NN on the 5th-generation tensor cores (tcgen05 / TMEM), sm_100a.
+// hamming_mma.cu -- brute-force Hamming 2-NN on the Hopper tensor cores (warpgroup wgmma, sm_90a).
 //
 // Reference behaviour (exact, same as hamming.cu): cv::BFMatcher(NORM_HAMMING).knnMatch(k = 2)
 //   opencv features2d/src/matchers.cpp:757 -> core/src/batch_distance.cpp:103-123 (batchDistHamming),
@@ -7,55 +7,49 @@
 // Why tensor cores: brute-force Hamming IS a contraction.  With every descriptor bit b expanded to the 8-bit value
 // 2b - 1 (+1 / -1), the dot product of two 256-element rows is  256 - 2 * hamming,  exactly (an int32, or a float whose
 // partial sums are all integers of magnitude <= 256).  So the N_q x N_t distance matrix is one 8-bit GEMM with K = 256, and the
-// integer pipes (which bound the LOP3/POPC kernel of hamming.cu at ~7.5e11 distances/s) are left with nothing but the top-2
-// selection.  Two operand kinds are built: kind::i8 (+-1 as int8, int32 accumulators; the default) and kind::f8f6f4 (+-1.0 as
-// E4M3, fp32 accumulators); the results are bit-identical (every value involved is an exactly representable integer).
-// Measured on B200 (profiles/r02a_knn_mma_i8_full.txt, tools/gpu_knn_mma_prof.py): once the epilogue was out of the way both
-// kinds run at the same rate, ~4 030 MAC/clk/SM (M = N = 128, cta_group::1: ~130 clk per instruction, tensor pipe ~49 % busy) --
-// the limit at this tile shape is the rate the MMA unit streams its two 32 KB operands from shared memory, not the arithmetic
-// kind.  N = 256 tiles (half the A re-reads per MAC), A kept in TMEM, or cta_group::2 are the next steps.
+// integer pipes (which bound the LOP3/POPC kernel of hamming.cu) are left with nothing but the top-2 selection.  Two operand
+// kinds are built: int8 (+-1 as s8, s32 accumulators; the default) and E4M3 (+-1.0, f32 accumulators); the results are
+// bit-identical (every value involved is an exactly representable integer).
 //
-// Shape of the kernel (one CTA per 256 query rows, 1 CTA / SM, 20 warps):
-//   warp 0   producer : bulk async copies (cp.async.bulk, SASS UBLKCP -- the TMA engine's 1-D mode) of pre-tiled 32 KB
-//                       operand blobs into a 4-stage shared-memory ring, completion on mbarriers
-//   warp 1   issuer   : one elected thread issues tcgen05.mma.kind::f8f6f4 / kind::i8 (SASS UTCQMMA / UTCIMMA), M = 128, N = 128, K = 32 per
-//                       instruction, 8 per K = 256, for TWO 128-row query tiles per train tile (every train byte that
-//                       leaves L2 feeds 256 query rows); accumulators live in TMEM, double-buffered (4 x 128 columns
-//                       = all 512), tcgen05.commit signals "smem stage free" and "accumulator ready"
-//   warp 2   TMEM allocator
-//   warps 4-19 epilogue: 2 query tiles x 4 TMEM lane quarters x 2 column halves.  tcgen05.ld (SASS LDTM) 2 x 32 columns in
-//                       flight; a row (= query) lives in one thread per column half, which reduces every 8 dot products to
-//                       their maximum (3-input max) and compares it with the dot product of its current second best; only
-//                       the groups that hit run the top-2 insertion, on packed keys hamming << 22 | index (one multiply-add
-//                       builds a key, three min / max insert it: OpenCV's strict '<' with ties to the lowest train index is
-//                       the unsigned order of those keys).  The two halves of a row are merged through shared memory.
-//                       (With 8 epilogue warps and a branchy insertion the MMAs waited on the epilogue 3/4 of the time and
-//                       int8 and FP8 operands ran equally slowly; 16 warps + the gated insertion moved the bound to the MMAs.)
+// Shape of the kernel (one CTA per 256 query rows, 1 CTA / SM, 17 warps):
+//   warps 0-15  consumers: 4 warpgroups, one per 64 query rows.  Per train tile each warpgroup issues 8
+//                       wgmma.mma_async m64n128k32 (K = 256) with both operands read from shared memory, waits for them,
+//                       hands the ring stage back, and runs the top-2 selection on the accumulators in its own registers
+//                       while the other warpgroups' MMAs keep the tensor cores busy.  In the accumulator fragment a thread
+//                       holds 32 columns of two rows; it reduces every 8 dot products of a row to their maximum and compares
+//                       it with the dot product of its current second best; only the groups that hit run the top-2
+//                       insertion, on packed keys hamming << 22 | index (one multiply-add builds a key, three min / max insert
+//                       it: OpenCV's strict '<' with ties to the lowest train index is the unsigned order of those keys).  The
+//                       four threads that share a row merge their pairs by shuffles at the end.
+//   warp 16     producer: bulk async copies (cp.async.bulk, the TMA engine's 1-D mode) of pre-tiled 32 KB operand blobs into
+//                       a 4-stage shared-memory ring, completion on mbarriers.
 // The operands are expanded from the packed 256-bit descriptors by knn2_expand_kernel straight into the shared-memory
-// image of a tile (UMMA canonical K-major layout), so the producer needs no tensor map and no swizzle pattern has to be
+// image of a tile (canonical K-major layout), so the producer needs no tensor map and no swizzle pattern has to be
 // matched by hand anywhere else.  Live queries of a batch are compacted on the way ([nbatch][qcap] slots, counts[b] live).
 #include "alva_common.cuh"
 #include "../../include/alva_b200.h"
 
 namespace {
 
-constexpr int TM = 128;                 // query rows per M tile (UMMA M)
-constexpr int TN = 128;                 // train rows per N tile (UMMA N)
+constexpr int TM = 128;                 // query rows per A tile (two wgmma M = 64 blocks)
+constexpr int TN = 128;                 // train rows per B tile (wgmma N)
+constexpr int WM = 64;                  // query rows per consumer warpgroup (wgmma M)
 constexpr int KBYTES = 256;             // int8 elements per expanded descriptor
 constexpr int BLOB = TM * KBYTES;       // one operand tile in shared memory: 32 KB
 constexpr int NSTAGE = 4;               // train-tile ring
-constexpr int EPI_WARP0 = 4;
-constexpr int EPI_WARPS = 16;            // 2 query tiles x 4 TMEM lane quarters x 2 column halves
-constexpr int NTHREADS = (EPI_WARP0 + EPI_WARPS) * 32;
+constexpr int CONS_WARPS = 16;          // 4 warpgroups x 64 query rows = 256 rows per CTA
+constexpr int PROD_WARP = CONS_WARPS;
+constexpr int NTHREADS = (CONS_WARPS + 1) * 32;   // + the producer warp
 constexpr uint32_t NONE = 0xffffffffu;
 constexpr int NEG = -(1 << 20);         // "no candidate yet" dot product
 
-// UMMA shared-memory matrix descriptor pieces, per layout mode (host-filled; kernel parameters so that a debugging run can
+// wgmma shared-memory matrix descriptor pieces, per layout mode (host-filled; kernel parameters so that a debugging run can
 // try a variant without a rebuild)
 struct MmaLayout {
-    uint32_t desc_hi;     // bits 32..63: stride byte offset >> 4 | version 1 (bit 46) | layout type (bits 61..63)
+    uint32_t desc_hi;     // bits 32..63: stride byte offset >> 4 (bits 32..45) | layout type (bits 62..63: 1 = 128-byte swizzle)
     uint32_t lbo16;       // leading byte offset >> 4 (bits 16..29)
     uint32_t koff[8];     // byte offset of K step j (32 int8 each) inside a tile
+    uint32_t moff;        // byte offset of query row 64 (the second warpgroup's rows) inside a tile
     int mode;             // 0: no swizzle ("interleaved" 8 x 16 B core matrices)   1: 128-byte swizzle
                           // 2: as 0 with the two offsets exchanged (debugging aid for the descriptor convention)
 };
@@ -74,49 +68,50 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void umma_i8(uint32_t d_tmem, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// D[64 x 128] (+)= A[64 x 32] * B[128 x 32]^T, both K-major in shared memory; the accumulator fragment stays in registers
+__device__ __forceinline__ void wgmma_i8(int (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem), "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "setp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, "
+        "%46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p;\n"
+        "}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]),
+          "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]),
+          "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]),
+          "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]),
+          "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]),
+          "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]),
+          "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]),
+          "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_f8(uint32_t d_tmem, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_e4m3(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem), "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "setp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, "
+        "%46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+          "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, int (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-          "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-          "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void bar_sync_named(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
 // ---------------------------------------------------------------------------------------------- operand expansion
 // offsets[b] = number of live queries in batches < b  (counts clamped to [0, qcap]); one small CTA
@@ -189,10 +184,7 @@ __global__ void __launch_bounds__(256) knn2_expand_kernel(const uint8_t* __restr
 
 // ---------------------------------------------------------------------------------------------- the matcher
 struct SmemBars {
-    uint64_t full[NSTAGE], empty[NSTAGE], tfull[2], tempty[2], afull;
-    uint32_t tmem_base;
-    uint32_t pad[3];
-    uint2 xchg[2 * TM];     // the two best keys of the upper column half of every row
+    uint64_t full[NSTAGE], empty[NSTAGE], afull;
 };
 
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, const MmaLayout& L) {
@@ -200,32 +192,39 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, const MmaLayout& L
     return (uint64_t)lo | ((uint64_t)L.desc_hi << 32);
 }
 
-// accumulator value type per operand kind, and the bit pattern <-> value conversions of the epilogue
+// accumulator value type per operand kind, and the value <-> key conversions of the epilogue
 template <int KIND> struct Acc;
 template <> struct Acc<0> {
     using T = int;
-    static __device__ __forceinline__ int from_bits(int b) { return b; }
     static __device__ __forceinline__ int neg() { return NEG; }
     static __device__ __forceinline__ int to_int(int v) { return v; }
     // (256 - dot) << 21 | idx as one multiply-add: dot * -(2^21) + ((256 << 21) + idx)  (idx < 2^22, (256 - dot) even)
     static __device__ __forceinline__ uint32_t key(int v, int idx) { return (uint32_t)v * 0xFFE00000u + ((256u << 21) + (uint32_t)idx); }
     static __device__ __forceinline__ int dot_of_key(uint32_t k) { return 256 - (int)(k >> 21); }   // NONE -> -1791: below every dot product
+    static __device__ __forceinline__ void mma(int (&d)[64], uint64_t da, uint64_t db, uint32_t acc) { wgmma_i8(d, da, db, acc); }
 };
 template <> struct Acc<1> {
     using T = float;
-    static __device__ __forceinline__ float from_bits(int b) { return __int_as_float(b); }
     static __device__ __forceinline__ float neg() { return (float)NEG; }
     // the accumulators are integer-valued floats of magnitude <= 256: adding 1.5 * 2^23 leaves the integer in the low mantissa bits
     static __device__ __forceinline__ int to_int(float v) { return __float_as_int(v + 12582912.0f) - 0x4B400000; }
     static __device__ __forceinline__ uint32_t key(float v, int idx) { return (uint32_t)to_int(v) * 0xFFE00000u + ((256u << 21) + (uint32_t)idx); }
     static __device__ __forceinline__ float dot_of_key(uint32_t k) { return (float)(256 - (int)(k >> 21)); }
+    static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) { wgmma_e4m3(d, da, db, acc); }
 };
+
+// the pair (k0, k1) of two smallest keys absorbs the pair (o0, o1)
+__device__ __forceinline__ void merge2(uint32_t& k0, uint32_t& k1, uint32_t o0, uint32_t o1) {
+    const uint32_t hi = max(k0, o0);
+    k0 = min(k0, o0);
+    k1 = min(min(k1, o1), hi);
+}
 
 template <int KIND>
 __global__ void __launch_bounds__(NTHREADS, 1)
 knn2_mma_kernel(const uint8_t* __restrict__ Aexp, const uint8_t* __restrict__ Bexp, const int32_t* __restrict__ rowmap,
                 const int32_t* __restrict__ total_ptr, int nrows, int nt, int ntiles, int tiles_per_chunk, int nchunks,
-                uint2* __restrict__ partial, const MmaLayout L, uint32_t idesc, int32_t* __restrict__ dbg) {
+                uint2* __restrict__ partial, const MmaLayout L, int32_t* __restrict__ dbg) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* sm = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* sA = sm;
@@ -240,18 +239,13 @@ knn2_mma_kernel(const uint8_t* __restrict__ Aexp, const uint8_t* __restrict__ Be
     const int nit = min(tiles_per_chunk, ntiles - tile0);     // >= 1 by construction of nchunks
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < NSTAGE; s++) { mbar_init(&B.full[s], 1); mbar_init(&B.empty[s], 1); }
-        for (int s = 0; s < 2; s++) { mbar_init(&B.tfull[s], 1); mbar_init(&B.tempty[s], EPI_WARPS); }
+        for (int s = 0; s < NSTAGE; s++) { mbar_init(&B.full[s], 1); mbar_init(&B.empty[s], CONS_WARPS); }
         mbar_init(&B.afull, 1);
         fence_barrier_init();
     }
-    if (warp == 2) tmem_alloc(&B.tmem_base, 512);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = B.tmem_base;
 
-    if (warp == 0) {
+    if (warp == PROD_WARP) {
         // ---------------------------------------------------------------- producer
         if (lane == 0) {
             mbar_arrive_expect_tx(&B.afull, 2 * BLOB);
@@ -267,112 +261,89 @@ knn2_mma_kernel(const uint8_t* __restrict__ Aexp, const uint8_t* __restrict__ Be
             }
             __syncwarp();
         }
-    } else if (warp == 1) {
-        // ---------------------------------------------------------------- MMA issuer
-        mbar_wait(&B.afull, 0);
-        for (int it = 0; it < nit; it++) {
-            const int s = it % NSTAGE, ph = (it / NSTAGE) & 1;
-            const int as = it & 1, aph = (it >> 1) & 1;
-            mbar_wait(&B.tempty[as], aph ^ 1);     // the epilogue has drained this accumulator stage
-            mbar_wait(&B.full[s], ph);             // the train tile has landed
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t a0 = smem_u32(sA), b0 = smem_u32(sB + s * BLOB);
+        return;
+    }
+
+    // -------------------------------------------------------------------- consumers: MMA + top-2 per query row
+    using A = Acc<KIND>;
+    using T = typename A::T;
+    const int g = warp >> 2;                                  // warpgroup: query rows [64 g, 64 g + 64) of the CTA
+    const int t = g >> 1;                                     // A tile
+    const int quad = lane & 3;
+    const int trow = (g & 1) * WM + (warp & 3) * 16 + (lane >> 2);   // row inside the A tile of accumulator row r0; r1 = r0 + 8
+    const uint32_t a0 = smem_u32(sA) + (uint32_t)t * BLOB + (uint32_t)(g & 1) * L.moff;
+    // Per thread and row: the two smallest keys seen, key = hamming << 22 | index = (256 - dot) << 21 | index -- the
+    // lexicographic (distance, index) order of OpenCV's insertion as ONE unsigned compare, so the insertion itself is three
+    // min / max and needs no order of arrival.  thr = the dot product of the current second best: a candidate can only
+    // matter if its dot product is strictly above it (its index is larger than everything this thread has seen).
+    uint32_t k0[2] = {NONE, NONE}, k1[2] = {NONE, NONE};
+    T thr[2] = {A::neg(), A::neg()};
+    T d[64];
 #pragma unroll
-                for (int t = 0; t < 2; t++) {
-                    const uint32_t d = tmem + (uint32_t)((as * 2 + t) * TN);
+    for (int i = 0; i < 64; i++) d[i] = T(0);
+
+    mbar_wait(&B.afull, 0);
+    for (int it = 0; it < nit; it++) {
+        const int s = it % NSTAGE, ph = (it / NSTAGE) & 1;
+        mbar_wait(&B.full[s], ph);                            // the train tile has landed
+        const uint32_t b0 = smem_u32(sB + s * BLOB);
+        wg_fence();
 #pragma unroll
-                    for (int j = 0; j < 8; j++) {
-                        const uint64_t da = make_desc(a0 + t * BLOB + L.koff[j], L), db = make_desc(b0 + L.koff[j], L);
-                        if (KIND) umma_f8(d, da, db, idesc, j > 0 ? 1u : 0u); else umma_i8(d, da, db, idesc, j > 0 ? 1u : 0u);
-                    }
-                }
-                umma_commit(&B.empty[s]);          // fires when the MMAs above have finished reading shared memory
-                umma_commit(&B.tfull[as]);         // ... and their results are in TMEM
-            }
-            __syncwarp();
+        for (int j = 0; j < 8; j++) A::mma(d, make_desc(a0 + L.koff[j], L), make_desc(b0 + L.koff[j], L), j > 0 ? 1u : 0u);
+        wg_commit();
+        wg_wait_all();
+        // the accumulators are in registers: hand the stage back to the producer before the selection work
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&B.empty[s]);
+
+        // fragment: d[4c + 2h + e] = D[r0 + 8h][8c + 2 quad + e], c < 16
+        if (dbg && pair == 0 && chunk == 0 && it == 0 && t == 0) {   // the raw dot products, before the tail is masked
+#pragma unroll
+            for (int i = 0; i < 64; i++) dbg[(trow + 8 * ((i >> 1) & 1)) * TN + 8 * (i >> 2) + 2 * quad + (i & 1)] = A::to_int(d[i]);
         }
-    } else if (warp >= EPI_WARP0) {
-        // ---------------------------------------------------------------- epilogue: top-2 per query row and column half
-        const int e = warp - EPI_WARP0;
-        const int lq = e & 3, t = (e >> 2) & 1, half = e >> 3;   // a warp may only touch TMEM lanes 32 * (warp % 4) ..; EPI_WARP0 % 4 == 0
-        const int trow = lq * 32 + lane;                         // row inside the 128-row tile
-        const int row = pair * 2 * TM + t * TM + trow;
-        using A = Acc<KIND>;
-        using T = typename A::T;
-        // Per thread: the two smallest keys seen, key = hamming << 22 | index = (256 - dot) << 21 | index -- the lexicographic
-        // (distance, index) order of OpenCV's insertion as ONE unsigned compare, so the insertion itself is three min / max and
-        // needs no order of arrival.  thr = the dot product of the current second best: a candidate can only matter if its dot
-        // product is strictly above it (its index is larger than everything this thread has seen).
-        uint32_t k0 = NONE, k1 = NONE;
-        T thr = A::neg();
-        auto max3 = [](T x, T y, T z) { return max(max(x, y), z); };
-        auto scan32 = [&](int (&vb)[32], int n0) {
-            T v[32];
+        const int n0 = (tile0 + it) * TN + 2 * quad;
+        if (n0 - 2 * quad + TN > nt) {                        // only the last train tile: columns past nt hold zero rows
 #pragma unroll
-            for (int j = 0; j < 32; j++) v[j] = A::from_bits(vb[j]);
-            const bool tail = n0 + 32 > nt;   // only the last train tile: columns past nt hold the dot products of zero rows
-            if (tail) {
-#pragma unroll
-                for (int j = 0; j < 32; j++) if (n0 + j >= nt) v[j] = A::neg();   // below every threshold: never opens a group
-            }
-#pragma unroll
-            for (int k = 0; k < 4; k++) {
-                const T g = max3(max3(v[8 * k], v[8 * k + 1], v[8 * k + 2]), max3(v[8 * k + 3], v[8 * k + 4], v[8 * k + 5]), max(v[8 * k + 6], v[8 * k + 7]));
-                if (g > thr) {
-#pragma unroll
-                    for (int j = 0; j < 8; j++) {
-                        uint32_t key = A::key(v[8 * k + j], n0 + 8 * k + j);
-                        if (tail && n0 + 8 * k + j >= nt) key = NONE;
-                        const uint32_t hi = max(k0, key);
-                        k0 = min(k0, key);
-                        k1 = min(k1, hi);
-                    }
-                    thr = A::dot_of_key(k1);
-                }
-            }
-        };
-        for (int it = 0; it < nit; it++) {
-            const int as = it & 1, aph = (it >> 1) & 1;
-            mbar_wait(&B.tfull[as], aph);
-            tc_fence_after();
-            const uint32_t taddr = tmem + ((uint32_t)(lq * 32) << 16) + (uint32_t)((as * 2 + t) * TN + half * (TN / 2));
-            const int n0 = (tile0 + it) * TN + half * (TN / 2);
-            int vb0[32], vb1[32];
-            tmem_ld32_issue(taddr, vb0);
-            tmem_ld32_issue(taddr + 32, vb1);
-            tmem_ld_wait();
-            // the accumulators are in registers: hand the stage back to the MMA issuer before the selection work
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&B.tempty[as]);
-            if (dbg && pair == 0 && chunk == 0 && it == 0 && t == 0) {
-#pragma unroll
-                for (int j = 0; j < 32; j++) {
-                    dbg[trow * TN + half * (TN / 2) + j] = A::to_int(A::from_bits(vb0[j]));
-                    dbg[trow * TN + half * (TN / 2) + 32 + j] = A::to_int(A::from_bits(vb1[j]));
-                }
-            }
-            scan32(vb0, n0);
-            scan32(vb1, n0 + 32);
+            for (int i = 0; i < 64; i++) if (n0 + 8 * (i >> 2) + (i & 1) >= nt) d[i] = A::neg();   // never opens a group
         }
-        // merge the two column halves of a row: the upper half hands its pair over through shared memory
-        if (half == 1) B.xchg[t * TM + trow] = make_uint2(k0, k1);
-        bar_sync_named(1, EPI_WARPS * 32);
-        if (half == 0 && row < total) {
-            const int slot = rowmap ? rowmap[row] : row;
-            if (slot >= 0) {
-                const uint2 o = B.xchg[t * TM + trow];
-                const uint32_t hi = max(k0, o.x);
-                const uint32_t b0 = min(k0, o.x);
-                const uint32_t b1 = min(min(k1, o.y), hi);
-                partial[(size_t)slot * nchunks + chunk] = make_uint2(b0, b1);
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+#pragma unroll
+            for (int k = 0; k < 4; k++) {                     // 8 columns of row r0 + 8h: c = 4k .. 4k + 3, e = 0, 1
+                T gmax = d[16 * k + 2 * h];
+#pragma unroll
+                for (int c = 0; c < 4; c++)
+#pragma unroll
+                    for (int e = 0; e < 2; e++) gmax = max(gmax, d[16 * k + 4 * c + 2 * h + e]);
+                if (gmax > thr[h]) {
+#pragma unroll
+                    for (int c = 0; c < 4; c++) {
+#pragma unroll
+                        for (int e = 0; e < 2; e++) {
+                            const int col = n0 + 8 * (4 * k + c) + e;
+                            const uint32_t key = col < nt ? A::key(d[16 * k + 4 * c + 2 * h + e], col) : NONE;
+                            const uint32_t hi = max(k0[h], key);
+                            k0[h] = min(k0[h], key);
+                            k1[h] = min(k1[h], hi);
+                        }
+                    }
+                    thr[h] = A::dot_of_key(k1[h]);
+                }
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem, 512);
+    // merge the four threads of a row (lanes 4 j .. 4 j + 3 hold disjoint columns of the same two rows)
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+#pragma unroll
+        for (int x = 1; x <= 2; x <<= 1)
+            merge2(k0[h], k1[h], __shfl_xor_sync(0xffffffffu, k0[h], x), __shfl_xor_sync(0xffffffffu, k1[h], x));
+        const int row = pair * 2 * TM + t * TM + trow + 8 * h;
+        if (quad == 0 && row < total) {
+            const int slot = rowmap ? rowmap[row] : row;
+            if (slot >= 0) partial[(size_t)slot * nchunks + chunk] = make_uint2(k0[h], k1[h]);
+        }
+    }
 }
 
 }  // namespace
@@ -389,24 +360,28 @@ static MmaLayout make_layout(int mode) {
     L.mode = mode;
     if (mode != 1) {
         // K-major, no swizzle: ((8, n), 2) : ((1, SBO), LBO) in 16-byte units -- core matrices of 8 rows x 16 B
-        L.lbo16 = (TM * 16) >> 4;                 // next 16-byte K chunk
-        L.desc_hi = (128u >> 4) | (1u << 14);     // SBO = next 8-row group; version 1; layout 0
+        L.lbo16 = (TM * 16) >> 4;                 // LBO = next 16-byte K chunk
+        L.desc_hi = 128u >> 4;                    // SBO = next 8-row group; layout 0
         for (int j = 0; j < 8; j++) L.koff[j] = (uint32_t)j * 2 * TM * 16;
-        if (mode == 2) { L.lbo16 = 128u >> 4; L.desc_hi = ((TM * 16u) >> 4) | (1u << 14); }
+        L.moff = WM * 16;
+        if (mode == 2) { L.lbo16 = 128u >> 4; L.desc_hi = (TM * 16u) >> 4; }
     } else {
-        // K-major, 128-byte swizzle: rows of 128 B, 8-row groups of 1024 B, two 128-byte K atoms per tile
+        // K-major, 128-byte swizzle: rows of 128 B, 8-row groups of 1024 B, two 128-byte K atoms per tile (LBO unused)
         L.lbo16 = 1;
-        L.desc_hi = (1024u >> 4) | (1u << 14) | (2u << 29);
+        L.desc_hi = (1024u >> 4) | (1u << 30);
         for (int j = 0; j < 8; j++) L.koff[j] = (uint32_t)(j >> 2) * TM * 128 + (uint32_t)(j & 3) * 32;
+        L.moff = WM * 128;
     }
     return L;
 }
 
-// true if the tensor-core path should serve this problem
+// true if the tensor-core path should serve this problem.  Measured on H100 (CUDA events, both paths on the same inputs): the
+// LOP3/POPC kernel is as fast or faster below ~4 M query x train pairs (2048 x 1024: 12.7 vs 13.6 us), the tensor cores win above
+// (4096 x 1024: 13.9 vs 14.6 us; 2048 x 10 000: 31 vs 46 us; 65 536 x 10 000: 317 vs 928 us).
 bool alva_knn2_mma_wanted(int nq, int nt) {
     if (alva_g_knn_mma == 2) return true;
     if (alva_g_knn_mma == 0) return false;
-    return nq >= 8192 && nt >= 1024;
+    return nq >= 1024 && nt >= 1024 && (long long)nq * nt >= (1LL << 22);
 }
 
 // q: [nq][32] (or [nbatch][qcap][32] with counts), t: [nt][32]; out: [nq][4] int32 as alva_k_hamming_knn2
@@ -451,20 +426,15 @@ int alva_knn2_mma_launch(alva_ctx* ctx, const uint8_t* q, int nq, const uint8_t*
     knn2_expand_kernel<<<a_blocks + b_blocks, 256, 0, ctx->stream>>>(q, offsets, nbatch, qcap, nq, Aexp, rowmap, a_blocks, t, nt, Bexp, L.mode, kind);
     ALVA_LAUNCH_CHECK(ctx);
 
-    // instruction descriptor (both operands K-major): N >> 3 at bit 17, M >> 4 at bit 24;
-    //   kind::i8     : D = S32 (bits 4-5 = 2), A = B = signed int8 (bits 7-9, 10-12 = 1)
-    //   kind::f8f6f4 : D = F32 (bits 4-5 = 1), A = B = E4M3 (bits 7-9, 10-12 = 0)
-    const uint32_t shape = ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
-    const uint32_t idesc = kind ? ((1u << 4) | shape) : ((2u << 4) | (1u << 7) | (1u << 10) | shape);
     const size_t smem = (size_t)(2 + NSTAGE) * BLOB + sizeof(SmemBars) + 1024;
     const dim3 grid(npairs, nchunks);
     const int32_t* total_ptr = counts ? offsets + nbatch : nullptr;
     if (kind) {
         ALVA_CUDA(cudaFuncSetAttribute(knn2_mma_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        knn2_mma_kernel<1><<<grid, NTHREADS, smem, ctx->stream>>>(Aexp, Bexp, rowmap, total_ptr, nq, nt, b_tiles, tiles_per_chunk, nchunks, partial, L, idesc, dbg_out);
+        knn2_mma_kernel<1><<<grid, NTHREADS, smem, ctx->stream>>>(Aexp, Bexp, rowmap, total_ptr, nq, nt, b_tiles, tiles_per_chunk, nchunks, partial, L, dbg_out);
     } else {
         ALVA_CUDA(cudaFuncSetAttribute(knn2_mma_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        knn2_mma_kernel<0><<<grid, NTHREADS, smem, ctx->stream>>>(Aexp, Bexp, rowmap, total_ptr, nq, nt, b_tiles, tiles_per_chunk, nchunks, partial, L, idesc, dbg_out);
+        knn2_mma_kernel<0><<<grid, NTHREADS, smem, ctx->stream>>>(Aexp, Bexp, rowmap, total_ptr, nq, nt, b_tiles, tiles_per_chunk, nchunks, partial, L, dbg_out);
     }
     ALVA_LAUNCH_CHECK(ctx);
     return alva_knn2_merge_launch(ctx, partial, nq, nchunks, out, counts, qcap);

@@ -28,7 +28,7 @@ using namespace alva_init;
 
 constexpr int INIT_THREADS = 128;
 constexpr int CHUNK = 32;   // hypotheses solved per round (one per thread of the first warp; the solver's local arrays make it
-                            // local-memory bound: 128 per round was measured slower, 3.8 vs 2.8 ms for a 100-iteration RANSAC)
+                            // local-memory bound, so more hypotheses per round mean more local-memory traffic per thread)
 
 struct EssentialParams {
     const double* bv1; const double* bv2; const int32_t* counts; int cap;

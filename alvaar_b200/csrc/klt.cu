@@ -1,4 +1,4 @@
-// klt.cu -- pyramidal Lucas-Kanade tracking of keypoints between consecutive frames, forward-backward checked, for sm_100a.
+// klt.cu -- pyramidal Lucas-Kanade tracking of keypoints between consecutive frames, forward-backward checked, for sm_90a.
 //
 // What is computed (bit-exact with the reference -- positions as float bit patterns, status, min-eigenvalue; the CPU
 // restatement is oracle/klt_oracle.c):

@@ -128,7 +128,7 @@ __global__ void __launch_bounds__(256) lc_score_kernel(const uint8_t* __restrict
         const int n = base_s;
         nmatch[p] = n;
         // the geometric check is run for the NEWEST keyframe of the step only (0 -> it returns at once for this pair): one round of
-        // the five-point RANSAC is ~2.8 ms of serial FP64 (Sturm / Newton root isolation: dependent Horner chains), longer than a
+        // the five-point RANSAC is serial FP64 (Sturm / Newton root isolation: dependent Horner chains) that outlasts a
         // pipeline step, and the temporal rule already asks the earlier events of the streak for match counts only
         // "enough" is relative as well: unrelated scenes still leave ~6 % of the keypoints as chance matches after the ratio test
         npair[p] = (e == K - 1 && n >= max(min_matches, nq / 8)) ? min(n, PAIR_CAP) : 0;
@@ -255,7 +255,7 @@ extern "C" int alva_lc_detect(alva_lc* lc, const uint8_t* gathered) { AlvaDevice
     // geometric check of every pair in one batch (count 0 -> immediate failure); intrinsics of the local block for the threshold
     const uint8_t* lb = gathered + (size_t)c.rank * K * lc->block_bytes;
     (void)lb;
-    // 32 hypotheses = one round of the RANSAC kernel (~0.7 ms; 100 were 2.8 ms per step -- longer than the step itself).  With ~70 %
+    // 32 hypotheses = one round of the RANSAC kernel (100 outlast a pipeline step).  With ~70 %
     // inliers among the putative matches one all-inlier 8-sample turns up in 32 draws 3 times out of 4; a miss only resets the
     // temporal counter of that stream for one keyframe.
     if (int e = alva_k_essential_5pt(ctx, lc->npair, PAIR_CAP, lc->bvl, lc->bvr, lc->npairs, 32, c.err_px, 0, c.fx_hint > 0 ? c.fx_hint : 500.f,

@@ -1,4 +1,4 @@
-// orb.cu -- ORB pre-blur and steered-BRIEF (rBRIEF-256) descriptors at given points, sm_100a.
+// orb.cu -- ORB pre-blur and steered-BRIEF (rBRIEF-256) descriptors at given points, sm_90a.
 //
 // Reference behaviour (bit-exact; CPU restatement in oracle/alva_oracle.c):
 //   FeatureExtractor::describeFeaturePoints   src/slam/src/feature_extractor.cpp:160-214
@@ -194,8 +194,7 @@ __global__ void __launch_bounds__(256) orb_describe_kernel(const uint8_t* __rest
                                                            uint8_t* __restrict__ desc, uint8_t* __restrict__ kept,
                                                            float* __restrict__ angles_out) {
     // the 256 test pairs as words (x0, y0, x1, y1), TRANSPOSED: pair 8 * lane + t sits at [t][lane], so the 8 loads of a warp are
-    // conflict-free (pair-major order put the lanes 32 bytes apart: 4 byte loads per pair, each 8-way bank conflicted --
-    // 81 % of this kernel's shared-memory wavefronts, profiles/r02_kernels_full.txt)
+    // conflict-free (pair-major order puts the lanes 32 bytes apart: 4 byte loads per pair, each 8-way bank conflicted)
     __shared__ uint32_t pat_s[8][32];
     for (int i = threadIdx.x; i < 256; i += blockDim.x) pat_s[i & 7][i >> 3] = reinterpret_cast<const uint32_t*>(c_pattern)[i];
     __syncthreads();

@@ -13,7 +13,7 @@
 //        Ceres trust-region LM (DENSE_QR)             same loop as ba.cu restates for the local BA
 //   caller VisualFrontend::computePose                src/slam/src/visual_frontend.cpp:245-417
 //
-// How (B200-first): the reference runs 100 hypotheses x (P3P + N distances + std::sort) serially.  Here
+// How: the reference runs 100 hypotheses x (P3P + N distances + std::sort) serially.  Here
 //   * the sampler's partial Fisher-Yates shuffle is the only serial piece (one thread, ~500 swaps in shared memory; its
 //     random numbers are a host-made table: std::mt19937 through libstdc++'s uniform_int_distribution is x >> 1);
 //   * all hypotheses of a problem are solved at once (thread per draw), kept in the reference's order;

@@ -1,4 +1,4 @@
-// system.cu -- `System`: the reference's public class (src/slam/src/system.hpp:19-56) re-hosted on the B200 hot path, plus its
+// system.cu -- `System`: the reference's public class (src/slam/src/system.hpp:19-56) re-hosted on the H100 hot path, plus its
 // C ABI (alva_system_*).  Same method names, argument meaning and return conventions as the reference so that embind.cpp /
 // system.js stay source-compatible (INTEGRATION.md):
 //
@@ -20,7 +20,7 @@
 //   triangulate  new map points at keyframes                      alva_k_triangulate                (multi_view_geometry.cpp:12-22)
 //   match_to_map local map -> keyframe matching                   alva_k_match_to_map               (mapper.cpp:354-587)
 //   ba_local     local bundle adjustment, both solves + flags     alva_k_ba_local                   (optimizer.cpp:251-359)
-// There is no CPU fallback: configure() fails without an sm_100 device.  Lens distortion: the JS shim always passes zeros
+// There is no CPU fallback: configure() fails without an sm_90 (H100) device.  Lens distortion: the JS shim always passes zeros
 // (system.js:84-141); non-zero coefficients are rejected rather than silently ignored.
 #include "alva_common.cuh"
 #include "../../include/alva_b200.h"

@@ -1,8 +1,9 @@
 #!/usr/bin/env python3
-"""bench.py -- headline benchmark of the B200-native per-frame visual-SLAM hot path.
+"""bench.py -- headline benchmark of the H100-native per-frame visual-SLAM hot path.
 
-    python bench.py --gpus N --steps K --warmup W            # this repo (CUDA, sm_100a)
+    python bench.py --gpus N --steps K --warmup W            # this repo (CUDA, sm_90a)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's own CPU code on the host cores
+    python bench.py ... --dump-outputs DIR                   # also write the last timed step's outputs as DIR/<name>.npy
 
 Metric (BASELINE.json): frames/sec @1280x720, 1000 ORB features/frame, 20-keyframe local BA; plus the achieved HBM
 bandwidth of the fused pyramid+FAST kernel against the measured copy peak (MEASURED_PEAKS.json).
@@ -35,7 +36,7 @@ sys.path.insert(0, ROOT)
 CONFIGS = {"c2": dict(w=1280, h=720, nfeat=1000, batch=64, name="c2_720p_stream+c4_local_ba"),
            "c3": dict(w=1920, h=1080, nfeat=2000, batch=32, name="c3_1080p_stream+c4_local_ba")}
 W, H = 1280, 720
-BATCH = 64            # frames per step: 64 x 3.69 MB RGBA = 236 MB per step, larger than the 126 MB L2
+BATCH = 64            # frames per step: 64 x 3.69 MB RGBA = 236 MB per step, larger than the 50 MB L2
 NFEAT = 1000
 WORKLOAD = "c2_720p_stream+c4_local_ba"
 MAP_SIZE = 10000
@@ -54,9 +55,6 @@ def select_config(name):
     c = CONFIGS[name]
     W, H, BATCH, NFEAT, WORKLOAD = c["w"], c["h"], c["batch"], c["nfeat"], c["name"]
     ALGO_BYTES_FRONTEND = 4 * W * H + W * H + ((W + 1) // 2) * ((H + 1) // 2)
-# dram__bytes_read.sum + dram__bytes_write.sum of one 64-frame front-end launch, from the committed `ncu --set full`
-# capture (profiles/r02_frontend_v2_full.txt).  Static by nature: a profiler cannot run inside bench.
-FRONTEND_DRAM_TRAFFIC_BYTES_B64 = 294_047_488   # dram__bytes_read.sum 235.976 MB + dram__bytes_write.sum 58.072 MB
 
 
 # sha256[:16] of the step's integer outputs (selected-feature counts + 2-NN match lists of all 64 frames) for the stream seeds
@@ -107,7 +105,7 @@ def read_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s)"
 
 
 class ClockSampler(threading.Thread):
@@ -322,7 +320,7 @@ def _workload_config(batch):
             "map_descriptors": MAP_SIZE, "ba": f"{BA_NKF} KF x {BA_NLM} landmarks x {BA_NLM * BA_OBS_PER_LM} obs, LM<={BA_ITERS}",
             "ba_every_n_frames": KF_INTERVAL,
             "ba_schedule": BA_SCHEDULE[0],
-            "l2_policy": f"inputs ({4 * W * H * batch / 1e6:.0f} MB/step) larger than L2 (126 MB)",
+            "l2_policy": f"inputs ({4 * W * H * batch / 1e6:.0f} MB/step) larger than L2 (50 MB)",
             "parallelism": "1 stream batch per GPU"}
 
 
@@ -486,6 +484,8 @@ def bench_b200(args, rank, world, local_rank):
         barrier()
         launches = ctx.launches - l0
         ms = ev0.elapsed_time(ev1)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, pipe, rank, world)
         graphs = pipe.graph_stats()
         # The dominant kernel's launch duration (roofline.achieved): CUDA events around the fused front-end launch of every
         # step of a SECOND pass of the same K steps, launched kernel by kernel -- the timed pass above replays CUDA graphs,
@@ -604,8 +604,6 @@ def bench_b200(args, rank, world, local_rank):
             "clocks": sampler.summary(),
             "roofline": {"kernel": "frontend_tile_kernel_v2<RGBA> (gray + pyramid L1 + FAST-9/NMS, fused)", "bound": "hbm",
                          "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": FRONTEND_DRAM_TRAFFIC_BYTES_B64 if (BATCH, W, H) == (64, 1280, 720) else None,
-                         "traffic_source": "ncu --set full of frontend_tile_kernel_v2, profiles/r02_frontend_v2_full.txt (bytes per launch)",
                          "peak_source": peak_src, "algorithmic_bytes_per_launch": ALGO_BYTES_FRONTEND * BATCH,
                          "launch_ms": fe_avg_ms,
                          "launch_ms_source": f"CUDA events around the launch in each of {len(fe)} steps of a second, kernel-by-kernel pass "
@@ -618,6 +616,32 @@ def bench_b200(args, rank, world, local_rank):
     print(json.dumps(line))
     if dist is not None:
         dist.destroy_process_group()
+
+
+def dump_outputs(out_dir, pipe, rank, world):
+    """What the timed path left in the pipeline's output buffers after its last step -- the arrays a caller of
+    alva_pipeline_step_dev reads -- as <out_dir>/<name>.npy (float32 / float64, integers exact).  Per-frame lists are zeroed
+    past each frame's count, so that two builds compare output for output whatever their buffers held beyond it."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    cnt = pipe.buffer("selcounts", (BATCH,), torch.int32).cpu().numpy()
+    live = np.arange(pipe.fcap)[None, :] < cnt[:, None]
+    per_frame = {"pts": ((BATCH, pipe.fcap, 2), torch.float32, np.float32),
+                 "desc": ((BATCH, pipe.fcap, 32), torch.uint8, np.float32),
+                 "matches": ((BATCH, pipe.fcap, 4), torch.int32, np.float64)}
+    out = {"nfeat": cnt.astype(np.float64)}
+    for name, (shape, tdt, ndt) in per_frame.items():
+        a = pipe.buffer(name, shape, tdt).cpu().numpy().astype(ndt)
+        a[~live] = 0
+        out[name] = a
+    if pipe.nprob:
+        out["ba_poses"] = pipe.buffer("ba_poses", (pipe.nprob, BA_NKF, 7), torch.float64).cpu().numpy()
+        out["ba_invd"] = pipe.buffer("ba_invd", (pipe.nprob, BA_NLM), torch.float64).cpu().numpy()
+        out["ba_summary"] = pipe.buffer("ba_summary", (pipe.nprob, 8), torch.float64).cpu().numpy()
+    assert sum(a.nbytes for a in out.values()) <= 64 << 20
+    suffix = f"_rank{rank}" if world > 1 else ""
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, name + suffix + ".npy"), a)
 
 
 def print_checksums():
@@ -843,7 +867,7 @@ def system_api_times_at(w, h, nf, with_reference):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--steps", type=int, default=20, help="timed steps (>= 1)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference", "reference-worker"])
     ap.add_argument("--config", default="c2", choices=sorted(CONFIGS), help="c2: 1280x720 / 1000 features (headline); c3: 1920x1080 / 2000 features")
@@ -852,8 +876,7 @@ def main():
     ap.add_argument("--print-checksums", action="store_true", help="print the output checksums of the step for the stream seeds 99..106 and exit")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-stage-stats", action="store_true",
-                    help="skip the explanatory per-stage / System-API timings after the timed region (profiling aid: ncu's "
-                         "serialisation of the 8 concurrent System threads corrupted its own heap at visit 9)")
+                    help="skip the explanatory per-stage / System-API timings after the timed region (profiling aid)")
     ap.add_argument("--no-ba-overlap", action="store_true", help="run the local BA after the frame stages instead of beside them")
     ap.add_argument("--no-loop-closure", action="store_true", help="N > 1: skip the NCCL keyframe-descriptor all-gather")
     ap.add_argument("--ba-lag", action="store_true",
@@ -862,7 +885,12 @@ def main():
     ap.add_argument("--frontend-ctas", type=int, default=0, help="A/B: resident front-end CTAs per SM (4 | 5)")
     ap.add_argument("--ba-ctl-threads", type=int, default=0, help="A/B: CTA size of the BA control kernels (256 | 512 | 1024)")
     ap.add_argument("--no-graphs", action="store_true", help="launch kernel by kernel instead of replaying CUDA graphs (profiling aid)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default="",
+                    help="write the outputs of the last timed step (feature counts, keypoints, descriptors, 2-NN matches, BA poses, "
+                         "inverse depths and summaries) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     select_config(args.config)
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     rank = int(os.environ.get("RANK", "0"))

@@ -1,4 +1,4 @@
-/* include/alva_b200.h -- C ABI of libalva_b200.so: the B200-native per-frame visual-SLAM hot path
+/* include/alva_b200.h -- C ABI of libalva_b200.so: the H100-native per-frame visual-SLAM hot path
  * behind AlvaAR's `System` API.
  *
  * Drop-in boundary (SURVEY.md section 8b).  The reference exposes its C++ `System` class to JavaScript
@@ -9,7 +9,7 @@
  *   alva_system_*   : one-to-one with System::{configure,reset,findCameraPose,findCameraPoseWithIMU,
  *                     findPlane,getFramePoints}  (system.hpp:28-38)
  *   alva_k_*        : kernel-level entry points for each stage of the hot path (device pointers),
- *                     the units the parity tests and the ncu captures address
+ *                     the units the parity tests address
  *   alva_h_*        : the same stages on HOST buffers (H2D + kernel + D2H inside the call) -- the
  *                     "e2e" leg of bench.py and what a non-CUDA host would call
  *
@@ -296,9 +296,9 @@ int alva_k_ba_local(alva_ctx*, int nprob, int nkf, int nlm, int nobs, const doub
  * "knn_qpw" = 4 | 8: queries a warp of the Hamming matcher keeps in registers (8: 128 registers / 16 warps per SM;
  * 4: 80 registers / 24 warps per SM).  Results are identical.
  * "knn_mma" = 0 | 1 | 2: the tensor-core formulation of the Hamming matcher (hamming_mma.cu: descriptors expanded to +-1
- * int8, tcgen05.mma.kind::i8, dot = 256 - 2 * distance): 0 never, 1 for large query sets (default), 2 always.  Results
- * are identical.  "knn_mma_kind" = 0 | 1: operand kind of that kernel (0: +-1 as int8, kind::i8, int32 accumulators -- default;
- * 1: +-1.0 as E4M3, kind::f8f6f4, fp32 accumulators; both run at the same measured rate at this tile shape).  "knn_mma_mode" = 0 | 1 | 2: its
+ * int8, wgmma s8 x s8 -> s32, dot = 256 - 2 * distance): 0 never, 1 for large query sets (default), 2 always.  Results
+ * are identical.  "knn_mma_kind" = 0 | 1: operand kind of that kernel (0: +-1 as int8, int32 accumulators -- default;
+ * 1: +-1.0 as E4M3, fp32 accumulators).  "knn_mma_mode" = 0 | 1 | 2: its
  * shared-memory operand layout (0 no swizzle, 1 128-byte swizzle, 2 debugging variant).
  * "frontend_variant" = 2 | 0: the fused front-end kernel (2: frontend_tile_kernel_v2, default; 0: the round-1 kernel, which
  * also serves geometries a TMA tensor map cannot express).  Results are identical.

@@ -60,7 +60,7 @@ def test_reference_class_shim_compiles_and_links():
 
 
 def test_python_system_binding_fails_loudly_without_a_gpu():
-    """alvaar_b200.System (the ctypes mirror of the reference's class): without an sm_100 device configure() must raise -- never a
+    """alvaar_b200.System (the ctypes mirror of the reference's class): without an sm_90 device configure() must raise -- never a
     silent CPU path."""
     import torch
     if torch.cuda.is_available():

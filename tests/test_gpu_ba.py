@@ -1,4 +1,4 @@
-"""GPU parity tests (B200): local BA through the C ABI vs the CPU oracle (itself pinned to ceres::Solve at 1e-14)
+"""GPU parity tests (H100): local BA through the C ABI vs the CPU oracle (itself pinned to ceres::Solve at 1e-14)
 and the golden Ceres solution.  FP64; tolerance 1e-4 relative on poses / inverse depths (north_star), plus equal
 iteration counts and termination reason."""
 import ctypes as C

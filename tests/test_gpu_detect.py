@@ -1,4 +1,4 @@
-"""GPU parity tests (B200): the reference's grid Shi-Tomasi detector + cornerSubPix through the C ABI vs the CPU oracle and
+"""GPU parity tests (H100): the reference's grid Shi-Tomasi detector + cornerSubPix through the C ABI vs the CPU oracle and
 the golden vectors dumped from the reference's own FeatureExtractor.  Bit-exact: integer maxima, order, count, adapted
 quality, and sub-pixel positions as float bit patterns."""
 import numpy as np

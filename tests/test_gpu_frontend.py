@@ -1,4 +1,4 @@
-"""GPU parity tests (B200): gray / pyramid / FAST-9 through the C ABI vs the CPU oracle and the golden vectors.
+"""GPU parity tests (H100): gray / pyramid / FAST-9 through the C ABI vs the CPU oracle and the golden vectors.
 Integer stages: bit-exact."""
 import numpy as np
 import pytest

@@ -1,4 +1,4 @@
-"""GPU parity tests (B200): the map-initialisation kernels (alva_k_essential_5pt, alva_k_triangulate) through the C ABI vs the
+"""GPU parity tests (H100): the map-initialisation kernels (alva_k_essential_5pt, alva_k_triangulate) through the C ABI vs the
 CPU oracle and the golden vectors dumped from the reference's own MultiViewGeometry + OpenGV.  Bars as in
 tests/test_oracle_init.py: RANSAC model 1e-9 and outlier set exact; refined pose inside the reference's own 1-ulp band and a
 cost no worse than the reference's; triangulated points 1e-11 relative."""

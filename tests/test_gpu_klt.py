@@ -1,4 +1,4 @@
-"""GPU parity tests (B200): pyramidal LK / forward-backward KLT through the C ABI vs the CPU oracle and the golden vectors
+"""GPU parity tests (H100): pyramidal LK / forward-backward KLT through the C ABI vs the CPU oracle and the golden vectors
 dumped from the reference's own FeatureTracker.  Bit-exact: tracked positions are compared as float bit patterns."""
 import numpy as np
 import pytest

@@ -1,4 +1,4 @@
-"""GPU tests (B200) of the cross-stream loop-closure detector (csrc/loopclosure.cu).  The reference has no loop closure
+"""GPU tests (H100) of the cross-stream loop-closure detector (csrc/loopclosure.cu).  The reference has no loop closure
 (SURVEY 8e: parity unpinned): what is checked is the wire format, determinism, detection of PLANTED revisits (the remote stream
 shows the same scene a few frames apart) with the temporal rule, and silence on unrelated streams."""
 import numpy as np

@@ -1,4 +1,4 @@
-"""GPU parity tests (B200): Mapper::matchToMap on flat device arenas through the C ABI vs the CPU oracle and the golden vectors
+"""GPU parity tests (H100): Mapper::matchToMap on flat device arenas through the C ABI vs the CPU oracle and the golden vectors
 dumped from the reference's own Mapper.  Exact: identical keypoint -> map point maps."""
 import numpy as np
 import pytest

@@ -1,4 +1,4 @@
-"""GPU parity tests (B200): ORB blur / rBRIEF descriptors / IC angle / Hamming 2-NN vs the oracle and goldens.
+"""GPU parity tests (H100): ORB blur / rBRIEF descriptors / IC angle / Hamming 2-NN vs the oracle and goldens.
 Descriptors and match indices are bit-exact; the blur is float arithmetic rounded to u8 and is checked bit-exact
 too (the kernel pins evaluation order and fusion exactly like the reference build it mirrors)."""
 import numpy as np
@@ -161,7 +161,7 @@ def knn_mma(gpu_ctx):
 @pytest.mark.parametrize("kind,mode", [(1, 0), (1, 1), (0, 0), (0, 1)])
 @pytest.mark.parametrize("nq,nt", [(1000, 10000), (1000, 1000), (7, 1), (1, 2), (33, 1025), (1000, 20000), (257, 129), (4100, 300)])
 def test_knn2_mma_vs_oracle(knn_mma, oracle, nq, nt, kind, mode):
-    """tcgen05 formulation (dot = 256 - 2 * distance; E4M3 / fp32 and int8 / int32 operand kinds, both shared-memory operand
+    """tensor-core (wgmma) formulation (dot = 256 - 2 * distance; E4M3 / fp32 and int8 / int32 operand kinds, both shared-memory operand
     layouts): bit-identical 2-NN lists incl. the tie rule"""
     assert knn_mma.L.alva_set_option(b"knn_mma_mode", mode) == 0
     assert knn_mma.L.alva_set_option(b"knn_mma_kind", kind) == 0

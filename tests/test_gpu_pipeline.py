@@ -1,4 +1,4 @@
-"""GPU parity test (B200): the whole per-frame hot path as one object (alva_pipeline_*) against the stage-by-stage
+"""GPU parity test (H100): the whole per-frame hot path as one object (alva_pipeline_*) against the stage-by-stage
 oracle: gray -> pyramid -> FAST -> retainBest -> ORB (IC angle) -> Hamming 2-NN -> local BA."""
 import ctypes as C
 

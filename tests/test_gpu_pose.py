@@ -1,4 +1,4 @@
-"""GPU parity tests (B200): batched P3P-LMedS and PnP through the C ABI vs the CPU oracle and the golden vectors dumped
+"""GPU parity tests (H100): batched P3P-LMedS and PnP through the C ABI vs the CPU oracle and the golden vectors dumped
 from the reference's own MultiViewGeometry.  fp64: pose within 1e-4 relative (BASELINE north_star; observed ~1e-12),
 inlier / outlier sets exact."""
 import numpy as np

@@ -1,4 +1,4 @@
-"""GPU tests (B200): the System facade (alva_system_*) -- the reference's public API (system.hpp:28-38) on the CUDA kernels --
+"""GPU tests (H100): the System facade (alva_system_*) -- the reference's public API (system.hpp:28-38) on the CUDA kernels --
 against the 100-frame trace of the reference's own System (tests/golden/system.npz `ref_*`) and against the same host-side state
 machine run over the CPU oracle (`cpu_*`, tools/make_golden_system.py).
 

@@ -1,4 +1,4 @@
-"""GPU test (B200), deliberately the LAST gpu test file in collection order: the experimental front-end instantiation
+"""GPU test (H100), deliberately the LAST gpu test file in collection order: the experimental front-end instantiation
 (alva_set_option("frontend_antipodal", 1)) against the default kernel.  Kept apart so that nothing else shares a process state
 with an experimental kernel before it has been seen on a GPU."""
 import numpy as np

@@ -1,5 +1,6 @@
 """CPU tests: the plain-C oracle against (a) the committed golden vectors dumped from the reference's own
-vendored OpenCV 4.5.5 (tools/make_golden.py) and (b) the live reference library when it exists in this tree."""
+vendored OpenCV 4.5.5 (tools/make_golden.py) and (b) the reference library on seeded inputs (live when it is built in this
+tree, else its stored outputs: tests/ref_golden.py)."""
 import ctypes as C
 
 import numpy as np
@@ -7,6 +8,7 @@ import pytest
 
 from conftest import P, golden
 from alvaar_b200 import synth
+from ref_golden import digest, ref_outputs
 
 
 def test_gray_golden(oracle):
@@ -115,31 +117,33 @@ def test_retain_best_threshold(oracle):
     assert oracle.orc_retain_best_threshold(P(xs), 10, 1) == 50
 
 
-# ---------------------------------------------------------------- live reference (build container only)
+# ---------------------------------------------------------------- the reference library (live, or its stored outputs)
 def test_live_reference_frontend(oracle, ref):
-    if ref is None:
-        pytest.skip("oracle/_ref/libalva_ref.so not built here")
     for (w, h, seed) in [(640, 480, 1), (333, 217, 2), (1280, 720, 3)]:
         rgba = synth.random_rgba(w, h, 1, seed)[0]
-        a, b = np.empty((h, w), np.uint8), np.empty((h, w), np.uint8)
-        ref.ref_gray(P(rgba), w, h, P(a))
-        oracle.orc_gray(P(rgba), w, h, P(b))
-        assert (a == b).all()
         img = synth.crop(w, h, 17 * seed, 29 * seed)
         dw, dh = (w + 1) // 2, (h + 1) // 2
-        a, b = np.empty((dh, dw), np.uint8), np.empty((dh, dw), np.uint8)
-        ref.ref_pyrdown(P(img), w, h, P(a))
+
+        def run_ref(R):
+            a, p = np.empty((h, w), np.uint8), np.empty((dh, dw), np.uint8)
+            R.ref_gray(P(rgba), w, h, P(a))
+            R.ref_pyrdown(P(img), w, h, P(p))
+            xa = np.zeros((w * h, 3), np.int32)
+            na = R.ref_fast(P(img), w, h, 20, 1, P(xa), w * h)
+            return {"gray": digest(a), "pyrdown": digest(p), "nfast": na, "fast": digest(xa[:na])}
+        want = ref_outputs(ref, f"frontend_{w}x{h}_{seed}", run_ref)
+        b = np.empty((h, w), np.uint8)
+        oracle.orc_gray(P(rgba), w, h, P(b))
+        assert (digest(b) == want["gray"]).all()
+        b = np.empty((dh, dw), np.uint8)
         oracle.orc_pyrdown(P(img), w, h, P(b))
-        assert (a == b).all()
-        xa, xb = np.zeros((w * h, 3), np.int32), np.zeros((w * h, 3), np.int32)
-        na = ref.ref_fast(P(img), w, h, 20, 1, P(xa), w * h)
+        assert (digest(b) == want["pyrdown"]).all()
+        xb = np.zeros((w * h, 3), np.int32)
         nb = oracle.orc_fast9(P(img), w, h, 20, 1, P(xb), w * h)
-        assert na == nb and (xa[:na] == xb[:nb]).all()
+        assert nb == int(want["nfast"]) and (digest(xb[:nb]) == want["fast"]).all()
 
 
 def test_live_reference_orb(oracle, ref):
-    if ref is None:
-        pytest.skip("oracle/_ref/libalva_ref.so not built here")
     w, h = 640, 480
     img = synth.crop(w, h, 100, 900)
     rng = np.random.default_rng(8)
@@ -148,12 +152,15 @@ def test_live_reference_orb(oracle, ref):
     ang = rng.uniform(0, 360, n).astype(np.float32)
     blur = np.empty_like(img)
     oracle.orc_orb_blur(P(img), w, h, 0, P(blur))
-    for angles in (None, ang):
-        da, ka = np.zeros((n, 32), np.uint8), np.zeros(n, np.uint8)
+    for tag, angles in (("upright", None), ("angles", ang)):
+        def run_ref(R):
+            da, ka = np.zeros((n, 32), np.uint8), np.zeros(n, np.uint8)
+            R.ref_orb_compute(P(img), w, h, P(pts), P(angles) if angles is not None else None, n, P(da), P(ka))
+            return {"kept": ka, "desc": digest(da[ka == 1])}
+        want = ref_outputs(ref, f"orb_compute_{tag}", run_ref)
         db, kb = np.zeros((n, 32), np.uint8), np.zeros(n, np.uint8)
-        ref.ref_orb_compute(P(img), w, h, P(pts), P(angles) if angles is not None else None, n, P(da), P(ka))
         oracle.orc_orb_describe(P(blur), w, h, P(pts), P(angles) if angles is not None else None, n, P(db), P(kb))
-        assert (ka == kb).all() and (da[ka == 1] == db[ka == 1]).all()
+        assert (want["kept"] == kb).all() and (want["desc"] == digest(db[kb == 1])).all()
 
 
 def _sorted_kp(kp, desc):
@@ -177,18 +184,20 @@ def test_orb_detect_composition_golden(oracle):
 
 @pytest.mark.parametrize("w,h,nfeat,thr", [(640, 480, 500, 20), (320, 240, 100, 30), (200, 150, 1000, 10)])
 def test_orb_detect_composition_vs_reference(oracle, ref, w, h, nfeat, thr):
-    if ref is None:
-        pytest.skip("oracle/_ref/libalva_ref.so not built here")
     img = synth.crop(w, h, 100 + w, 50 + h // 2)
     assert img.shape == (h, w)
     kp, d = np.zeros((8000, 4), np.float32), np.zeros((8000, 32), np.uint8)
     n = oracle.orc_orb_detect(P(img), w, h, nfeat, thr, 0, P(kp), P(d), 8000)
-    rk, rd = np.zeros((8000, 5), np.float32), np.zeros((8000, 32), np.uint8)
-    nr = ref.ref_orb_detect(P(img), w, h, nfeat, thr, P(rk), P(rd), 8000)
-    assert n == nr and n > 20
-    gk, gd = _sorted_kp(rk[:nr], rd[:nr])
-    assert (kp[:n].view(np.uint32) == np.ascontiguousarray(gk[:, :4]).view(np.uint32)).all()
-    assert (d[:n] == gd).all()
+
+    def run_ref(R):
+        rk, rd = np.zeros((8000, 5), np.float32), np.zeros((8000, 32), np.uint8)
+        nr = R.ref_orb_detect(P(img), w, h, nfeat, thr, P(rk), P(rd), 8000)
+        gk, gd = _sorted_kp(rk[:nr], rd[:nr])
+        return {"n": nr, "kp": digest(np.ascontiguousarray(gk[:, :4]).view(np.uint32)), "desc": digest(gd)}
+    want = ref_outputs(ref, f"orb_detect_{w}x{h}_{nfeat}_{thr}", run_ref)
+    assert n == int(want["n"]) and n > 20
+    assert (digest(kp[:n].view(np.uint32)) == want["kp"]).all()
+    assert (digest(d[:n]) == want["desc"]).all()
 
 
 def test_scharr_golden(oracle):
@@ -204,12 +213,14 @@ def test_scharr_golden(oracle):
 
 @pytest.mark.parametrize("w,h", [(640, 480), (33, 17), (7, 5), (1, 9), (9, 1), (2, 2)])
 def test_scharr_vs_reference(oracle, ref, w, h):
-    if ref is None:
-        pytest.skip("oracle/_ref/libalva_ref.so not built here")
     img = np.ascontiguousarray(synth.crop(max(w, 16), max(h, 16), 40, 60)[:h, :w])
-    lv, dv = np.zeros((h, w), np.uint8), np.zeros((h, w, 2), np.int16)
-    LP, DP = (C.c_void_p * 4)(lv.ctypes.data, None, None, None), (C.c_void_p * 4)(dv.ctypes.data, None, None, None)
-    ref.ref_build_pyramid(P(img), w, h, 3, 0, LP, DP)
+
+    def run_ref(R):
+        lv, dv = np.zeros((h, w), np.uint8), np.zeros((h, w, 2), np.int16)
+        LP, DP = (C.c_void_p * 4)(lv.ctypes.data, None, None, None), (C.c_void_p * 4)(dv.ctypes.data, None, None, None)
+        R.ref_build_pyramid(P(img), w, h, 3, 0, LP, DP)
+        return {"l0": digest(lv), "d0": digest(dv)}
+    want = ref_outputs(ref, f"scharr_{w}x{h}", run_ref)
     out = np.zeros((h, w, 2), np.int16)
     oracle.orc_scharr(P(img), w, h, P(out))
-    assert (lv == img).all() and (out == dv).all()
+    assert (digest(img) == want["l0"]).all() and (digest(out) == want["d0"]).all()

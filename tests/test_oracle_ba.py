@@ -1,5 +1,5 @@
-"""CPU tests: the BA oracle (oracle/ba_oracle.c) against ceres::Solve + AlvaAR's cost functor (live reference when
-built in this tree) and the committed golden solution."""
+"""CPU tests: the BA oracle (oracle/ba_oracle.c) against ceres::Solve + AlvaAR's cost functor (live when the reference is
+built in this tree, else its stored outputs: tests/ref_golden.py) and the committed golden solution."""
 import ctypes as C
 
 import numpy as np
@@ -7,6 +7,7 @@ import pytest
 
 from conftest import P, golden
 from alvaar_b200 import synth
+from ref_golden import ref_outputs
 
 
 def solve_with(L, prefix, pb, max_iter=5, huber=None):
@@ -23,26 +24,41 @@ def solve_with(L, prefix, pb, max_iter=5, huber=None):
 
 
 def test_se3_plus_and_functor_vs_reference(oracle, ref):
-    if ref is None:
-        pytest.skip("oracle/_ref/libalva_ref.so not built here")
     rng = np.random.default_rng(0)
     pb = synth.make_ba_problem(6, 50, 3, seed=1)
+    xs, ds = [], []
     for _ in range(200):
-        x = pb["poses"][rng.integers(0, 6)].copy()
-        d = rng.normal(0, 0.05, 6) * (rng.random() < 0.9)
-        a, b = np.zeros(7), np.zeros(7)
-        ref.ref_se3_plus(P(x), P(d), P(a))
-        oracle.orc_se3_plus(P(x), P(d), P(b))
-        assert np.allclose(a, b, rtol=0, atol=1e-14)
-    ref.ref_ba_evaluate.restype = C.c_int
-    oracle.orc_ba_evaluate.restype = C.c_int
-    for o in range(len(pb["obs_kf"])):
+        xs.append(pb["poses"][rng.integers(0, 6)].copy())
+        ds.append(rng.normal(0, 0.05, 6) * (rng.random() < 0.9))
+    nobs = len(pb["obs_kf"])
+
+    def inputs(o):
         l = pb["obs_lm"][o]
         obs = np.array([*pb["obs_uv"][o], *pb["anch_uv"][l]])
-        anch, pose = pb["poses"][pb["anch_kf"][l]].copy(), pb["poses"][pb["obs_kf"][o]].copy()
-        ra, Ja7, Jp7, Jda, c2a = np.zeros(2), np.zeros(14), np.zeros(14), np.zeros(2), np.zeros(1)
+        return l, obs, pb["poses"][pb["anch_kf"][l]].copy(), pb["poses"][pb["obs_kf"][o]].copy()
+
+    def run_ref(R):
+        plus = np.zeros((200, 7))
+        for i in range(200):
+            R.ref_se3_plus(P(xs[i]), P(ds[i]), P(plus[i]))
+        R.ref_ba_evaluate.restype = C.c_int
+        out = {"plus": plus, "ok": np.zeros(nobs, np.int32), "r": np.zeros((nobs, 2)), "Ja": np.zeros((nobs, 14)),
+               "Jp": np.zeros((nobs, 14)), "Jd": np.zeros((nobs, 2)), "c2": np.zeros((nobs, 1))}
+        for o in range(nobs):
+            l, obs, anch, pose = inputs(o)
+            out["ok"][o] = R.ref_ba_evaluate(P(pb["calib"]), P(anch), P(pose), C.c_double(pb["invd"][l]), P(obs), P(out["r"][o]),
+                                             P(out["Ja"][o]), P(out["Jp"][o]), P(out["Jd"][o]), P(out["c2"][o]))
+        return out
+    want = ref_outputs(ref, "se3_plus_and_functor", run_ref)
+    for i in range(200):
+        b = np.zeros(7)
+        oracle.orc_se3_plus(P(xs[i]), P(ds[i]), P(b))
+        assert np.allclose(want["plus"][i], b, rtol=0, atol=1e-14)
+    oracle.orc_ba_evaluate.restype = C.c_int
+    for o in range(nobs):
+        l, obs, anch, pose = inputs(o)
+        fa, ra, Ja7, Jp7, Jda, c2a = want["ok"][o], want["r"][o], want["Ja"][o], want["Jp"][o], want["Jd"][o], want["c2"][o]
         rb, Ja6, Jp6, Jdb, c2b = np.zeros(2), np.zeros(12), np.zeros(12), np.zeros(2), np.zeros(1)
-        fa = ref.ref_ba_evaluate(P(pb["calib"]), P(anch), P(pose), C.c_double(pb["invd"][l]), P(obs), P(ra), P(Ja7), P(Jp7), P(Jda), P(c2a))
         fb = oracle.orc_ba_evaluate(P(pb["calib"]), P(anch), P(pose), C.c_double(pb["invd"][l]), P(obs), P(rb), P(Ja6), P(Jp6), P(Jdb), P(c2b))
         assert fa == fb
         assert np.allclose(ra, rb, rtol=1e-12, atol=1e-10)
@@ -57,10 +73,10 @@ def test_se3_plus_and_functor_vs_reference(oracle, ref):
 def test_solve_vs_ceres(oracle, ref, nkf, nlm, k, seed, huber):
     """Same iteration count, termination, and poses / inverse depths within 1e-4 relative (north_star tolerance;
     observed agreement is ~1e-9) of ceres::Solve(SPARSE_SCHUR, LM, <=5 it, Huber)."""
-    if ref is None:
-        pytest.skip("oracle/_ref/libalva_ref.so not built here")
     pb = synth.make_ba_problem(nkf, nlm, k, seed=seed)
-    ok_a, pa, da, sa, ca = solve_with(ref, "ref", pb, huber=huber)
+    want = ref_outputs(ref, f"ba_solve_{nkf}_{nlm}_{k}_{seed}_{huber}",
+                       lambda R: dict(zip(("ok", "poses", "invd", "summary", "costs"), solve_with(R, "ref", pb, huber=huber))))
+    ok_a, pa, da, sa, ca = (want[k] for k in ("ok", "poses", "invd", "summary", "costs"))
     ok_b, pb_, db, sb, cb = solve_with(oracle, "orc", pb, huber=huber)
     assert ok_a == ok_b == 1
     assert sa[3] == sb[3] and sa[2] == sb[2] and sa[4] == sb[4], (sa, sb)
@@ -100,10 +116,10 @@ def local_with(L, prefix, pb, max_iter=5, thr=5.9915):
 def test_local_ba_vs_ceres(oracle, ref, nkf, nlm, k, seed):
     """Optimizer::localBA steps 2-4 (solve, drop chi2 / negative-depth outliers at the functors' last evaluation,
     conditional second solve, second flagging): identical outlier sets and iteration counts, solution to 1e-12."""
-    if ref is None:
-        pytest.skip("oracle/_ref/libalva_ref.so not built here")
     pb = synth.make_ba_problem(nkf, nlm, k, seed=seed)
-    ra, pa, da, fa, sa = local_with(ref, "ref", pb)
+    want = ref_outputs(ref, f"ba_local_{nkf}_{nlm}_{k}_{seed}",
+                       lambda R: dict(zip(("nbad", "poses", "invd", "flags", "summary"), local_with(R, "ref", pb))))
+    ra, pa, da, fa, sa = (want[k] for k in ("nbad", "poses", "invd", "flags", "summary"))
     rb, pb_, db, fb, sb = local_with(oracle, "orc", pb)
     assert ra == rb and ra > 0 and (fa == fb).all()
     assert (sa[[2, 3, 4, 7, 8, 9]] == sb[[2, 3, 4, 7, 8, 9]]).all()
@@ -118,9 +134,8 @@ def test_local_ba_no_outliers_skips_second_solve(oracle, ref):
     ok, p0, d0, s0, _ = solve_with(oracle, "orc", pb)
     assert nb == 0 and (f1 == 0).all() and (s1[5:] == 0).all()
     assert (p1 == p0).all() and (d1 == d0).all()
-    if ref is not None:
-        nr, pr, dr, fr, sr = local_with(ref, "ref", pb, thr=1e9)
-        assert nr == 0 and np.abs(pr - p1).max() < 1e-11
+    want = ref_outputs(ref, "ba_local_no_outliers", lambda R: dict(zip(("nbad", "poses"), local_with(R, "ref", pb, thr=1e9)[:2])))
+    assert want["nbad"] == 0 and np.abs(want["poses"] - p1).max() < 1e-11
 
 
 def test_local_ba_golden_ceres(oracle):

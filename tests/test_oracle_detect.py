@@ -8,6 +8,7 @@ import pytest
 from conftest import P, golden
 from alvaar_b200 import synth
 from detect_util import oracle_detect, random_cur
+from ref_golden import ref_outputs
 
 
 def bits(a):
@@ -33,19 +34,24 @@ def test_detect_golden(oracle, tag):
 
 @pytest.mark.parametrize("w,h,cs,seed,ncur", [(640, 480, 40, 5, 0), (640, 480, 40, 6, 80), (1280, 720, 40, 7, 250), (400, 300, 30, 8, 20)])
 def test_detect_live_reference(oracle, ref, w, h, cs, seed, ncur):
-    if ref is None or not hasattr(ref, "ref_detect_points"):
-        pytest.skip("oracle/_ref/libalva_ref.so (with FeatureExtractor) not built in this tree")
     fr, _ = synth.make_frames(1, w, h, seed=seed, rgba=False)
     img = np.ascontiguousarray(fr[0])
     cur = random_cur(w, h, ncur, seed)
     roi = np.array([20, 20, w - 40, h - 40], np.int32)
-    ref.ref_detect_points.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_double, C.c_void_p, C.c_int]
-    for q0 in (0.001, 0.00002):
-        want = np.zeros((4096, 2), np.float32)
-        n = ref.ref_detect_points(P(img), w, h, cs, P(cur), ncur, P(roi), q0, P(want), 4096)
+
+    def run_ref(R):
+        R.ref_detect_points.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_double, C.c_void_p, C.c_int]
+        out = {}
+        for i, q0 in enumerate((0.001, 0.00002)):
+            pts = np.zeros((4096, 2), np.float32)
+            n = R.ref_detect_points(P(img), w, h, cs, P(cur), ncur, P(roi), q0, P(pts), 4096)
+            out[f"pts{i}"] = pts[:n]
+        return out
+    want = ref_outputs(ref, f"detect_{w}x{h}_{cs}_{seed}_{ncur}", run_ref)
+    for i, q0 in enumerate((0.001, 0.00002)):
         pts, _, _ = oracle_detect(oracle, img, cs, cur, roi, q0)
-        assert len(pts) == n
-        assert (bits(pts) == bits(want[:n])).all()
+        assert len(pts) == len(want[f"pts{i}"])
+        assert (bits(pts) == bits(want[f"pts{i}"])).all()
 
 
 def test_quality_adaptation(oracle):
@@ -72,17 +78,20 @@ def test_occupied_cells_are_skipped(oracle):
 
 def test_corner_subpix_live_reference_with_border_points(oracle, ref):
     """cv::cornerSubPix incl. the replicate-border sampling path (points within 5 px of the frame)."""
-    if ref is None or not hasattr(ref, "ref_corner_subpix"):
-        pytest.skip("oracle/_ref/libalva_ref.so not built in this tree")
     w, h, n = 320, 240, 600
     fr, _ = synth.make_frames(1, w, h, seed=4, rgba=False)
     img = np.ascontiguousarray(fr[0])
     rng = np.random.default_rng(2)
     pts = np.stack([rng.uniform(0, w - 1, n), rng.uniform(0, h - 1, n)], 1).astype(np.float32)
     pts[:50, 0] = rng.uniform(0, 5, 50); pts[50:100, 1] = rng.uniform(h - 6, h - 1, 50); pts[100:150, 0] = rng.uniform(w - 6, w - 1, 50)
-    a, b = pts.copy(), pts.copy()
-    ref.ref_corner_subpix.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_double]
-    oracle.orc_corner_subpix.argtypes = ref.ref_corner_subpix.argtypes
-    ref.ref_corner_subpix(P(img), w, h, P(a), n, 3, 30, 0.01)
+    argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_double]
+
+    def run_ref(R):
+        a = pts.copy()
+        R.ref_corner_subpix.argtypes = argtypes
+        R.ref_corner_subpix(P(img), w, h, P(a), n, 3, 30, 0.01)
+        return {"pts": a}
+    a, b = ref_outputs(ref, "corner_subpix_border", run_ref)["pts"], pts.copy()
+    oracle.orc_corner_subpix.argtypes = argtypes
     oracle.orc_corner_subpix(P(img), w, h, P(b), n, 3, 30, 0.01)
     assert (bits(a) == bits(b)).all()

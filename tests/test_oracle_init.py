@@ -16,6 +16,7 @@ import pytest
 
 from conftest import P, golden
 from init_util import TAGS, host_core, orc_essential, pose_error, ransac_threshold, ref_essential, refine_cost
+from ref_golden import ref_outputs
 from alvaar_b200 import synth
 
 
@@ -117,21 +118,26 @@ def test_live_reference_agreement(oracle, ref):
     Sturm.cpp:296-330, fivept_nister/modules.cpp:518-545) or picked a neighbouring hypothesis with the same inlier count; its
     null-space basis comes out of a Jacobi SVD of a rank-deficient matrix and cannot be reproduced, so those stay.  After the
     refinement the poses agree whenever the outlier sets do (same band as the goldens)."""
-    if ref is None:
-        pytest.skip("oracle/_ref not built here")
     bad_set = bad_model = 0
     for seed in range(30):
         n = [60, 150, 192, 400][seed % 4]
         pr = synth.make_twoview_problem(n=n, seed=100 + seed, noise_px=[0.1, 0.3, 0.6][seed % 3], outlier_frac=[0.05, 0.15, 0.3][(seed // 3) % 3])
         K = pr["K"].astype(np.float32)
-        ok_r, Rt_r, o_r = ref_essential(ref, pr["bv1"], pr["bv2"], K, 0)
+
+        def run_ref(R):
+            out = {}
+            for opt in (0, 1):
+                out[f"ok{opt}"], out[f"Rt{opt}"], out[f"outl{opt}"] = ref_essential(R, pr["bv1"], pr["bv2"], K, opt)
+            return out
+        r = ref_outputs(ref, f"essential_{seed}", run_ref)
+        ok_r, Rt_r, o_r = r["ok0"], r["Rt0"], r["outl0"]
         ok_o, Rt_o, o_o, _ = orc_essential(oracle, pr["bv1"], pr["bv2"], K, 0)
         assert ok_r == ok_o
         if (o_r != o_o).any():
             bad_set += 1
             continue
         bad_model += np.abs(Rt_r - Rt_o).max() > 1e-9
-        ok_r, Rt_r, o_r = ref_essential(ref, pr["bv1"], pr["bv2"], K, 1)
+        ok_r, Rt_r, o_r = r["ok1"], r["Rt1"], r["outl1"]
         ok_o, Rt_o, o_o, _ = orc_essential(oracle, pr["bv1"], pr["bv2"], K, 1)
         dR, dt = pose_error(Rt_o, Rt_r)
         assert dR < 2e-3 and dt < 5e-3, (seed, dR, dt)
@@ -142,16 +148,14 @@ def test_live_reference_agreement(oracle, ref):
 def test_reference_refinement_is_noise_limited(ref):
     """The finding that sets the tolerance of the refined pose: a 1-ulp change of the bearing vectors moves the REFERENCE's own
     refined rotation by > 1e-7 (up to 1e-3) -- far more than the 1e-16 an exact minimiser would move."""
-    if ref is None:
-        pytest.skip("oracle/_ref not built here")
     rng = np.random.default_rng(0)
     moved = []
     for seed in range(6):
         pr = synth.make_twoview_problem(n=150, seed=seed)
         K = pr["K"].astype(np.float32)
-        _, A, _ = ref_essential(ref, pr["bv1"], pr["bv2"], K, 1)
         b1 = pr["bv1"] * (1 + rng.choice([-1, 0, 1], pr["bv1"].shape) * 2.2e-16)
         b2 = pr["bv2"] * (1 + rng.choice([-1, 0, 1], pr["bv2"].shape) * 2.2e-16)
-        _, B, _ = ref_essential(ref, b1, b2, K, 1)
-        moved.append(max(pose_error(A, B)))
+        r = ref_outputs(ref, f"essential_ulp_{seed}", lambda R: {"A": ref_essential(R, pr["bv1"], pr["bv2"], K, 1)[1],
+                                                                "B": ref_essential(R, b1, b2, K, 1)[1]})
+        moved.append(max(pose_error(r["A"], r["B"])))
     assert max(moved) > 1e-7

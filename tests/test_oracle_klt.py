@@ -9,6 +9,7 @@ import pytest
 from conftest import P, golden
 from alvaar_b200 import synth
 from klt_util import build_pyramid, klt_points, oracle_fb_klt, oracle_klt_lk
+from ref_golden import ref_outputs
 
 
 def bits(a):
@@ -45,20 +46,26 @@ def test_klt_lk_golden(oracle, levels, ui):
 
 @pytest.mark.parametrize("w,h,seed", [(161, 91, 2), (320, 240, 7)])
 def test_fb_klt_live_reference(oracle, ref, w, h, seed):
-    if ref is None:
-        pytest.skip("oracle/_ref/libalva_ref.so not built in this tree")
     fr, _ = synth.make_frames(2, w, h, seed=seed, rgba=False)
     a, b = np.ascontiguousarray(fr[0]), np.ascontiguousarray(fr[1])
     n = 250
     pts, pri = klt_points(w, h, n, seed)
-    L = ref.ref_build_pyramid(P(a), w, h, 9, 3, None, None)
+
+    def run_ref(R):
+        out = {"nlevels": R.ref_build_pyramid(P(a), w, h, 9, 3, None, None)}
+        R.ref_fb_klt.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
+                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
+        for levels in (1, 3):
+            q1, g1 = pri.copy(), np.zeros(n, np.uint8)
+            R.ref_fb_klt(P(a), P(b), w, h, 9, 3, levels, 30.0, 0.5, P(pts), P(q1), P(g1), n)
+            out[f"pts{levels}"], out[f"good{levels}"] = q1, g1
+        return out
+    want = ref_outputs(ref, f"fb_klt_{w}x{h}_{seed}", run_ref)
+    L = int(want["nlevels"])
     pa, da = build_pyramid(oracle, a, L)
     pb, db = build_pyramid(oracle, b, L)
-    ref.ref_fb_klt.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
-                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
     for levels in (1, 3):
-        q1, g1 = pri.copy(), np.zeros(n, np.uint8)
-        ref.ref_fb_klt(P(a), P(b), w, h, 9, 3, levels, 30.0, 0.5, P(pts), P(q1), P(g1), n)
+        q1, g1 = want[f"pts{levels}"], want[f"good{levels}"]
         q2, g2 = oracle_fb_klt(oracle, pa, da, pb, db, w, h, levels, pts, pri)
         assert (g1 == g2).all() and g1.sum() > 50
         assert (bits(q1) == bits(q2)).all()

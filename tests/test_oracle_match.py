@@ -6,6 +6,7 @@ import pytest
 from conftest import golden
 from alvaar_b200 import synth
 from match_util import oracle_match, reference_match
+from ref_golden import ref_outputs
 
 
 def problem(seed):
@@ -31,12 +32,14 @@ def test_match_golden(oracle, seed, nkp3d):
 
 @pytest.mark.parametrize("seed", [11, 12, 13, 14, 15, 16])
 def test_match_live_reference(oracle, ref, seed):
-    if ref is None or not hasattr(ref, "ref_match_to_map"):
-        pytest.skip("oracle/_ref/libalva_ref.so (full AlvaAR build) not present in this tree")
     p = synth.make_match_problem(seed, n_frame_kp=120 + 13 * (seed % 5), n_local=300 + 37 * (seed % 7), dup_frac=0.5)
     for nk in (100, 5):
-        order, want = reference_match(ref, p, nk)
-        assert oracle_match(oracle, p, order, nk) == want and len(want) > 30
+        def run_ref(R):
+            order, m = reference_match(R, p, nk)
+            return {"order": order, "kp": np.array(list(m.keys()), np.int32), "mp": np.array(list(m.values()), np.int32)}
+        r = ref_outputs(ref, f"match_to_map_{seed}_{nk}", run_ref)
+        want = dict(zip(r["kp"].tolist(), r["mp"].tolist()))
+        assert oracle_match(oracle, p, r["order"], nk) == want and len(want) > 30
 
 
 def test_match_order_decides_ties(oracle):

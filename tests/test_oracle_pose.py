@@ -8,6 +8,7 @@ import pytest
 
 from conftest import P, golden
 from pose_util import make_pose_problem
+from ref_golden import ref_outputs
 
 f32 = C.c_float
 HUBER = float(np.sqrt(np.float32(5.9915)))   # ceresPnP: std::sqrt(float chi2th) (multi_view_geometry.cpp:147)
@@ -70,19 +71,25 @@ def test_sampler_sequence_is_mt19937_shift(oracle):
 
 @pytest.mark.parametrize("n,seed,of", [(120, 11, 0.2), (700, 12, 0.35), (9, 13, 0.0)])
 def test_pose_live_reference(oracle, ref, n, seed, of):
-    if ref is None or not hasattr(ref, "ref_p3p_lmeds"):
-        pytest.skip("oracle/_ref/libalva_ref.so (with OpenGV) not built in this tree")
     pr = make_pose_problem(n, seed, outlier_frac=of)
     K32 = pr["K"].astype(np.float32)
-    ref.ref_p3p_lmeds.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, f32, f32, f32, C.c_void_p, C.c_void_p]
-    ref.ref_pnp.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, f32, C.c_int, C.c_int, f32, f32, f32, f32, C.c_void_p]
-    T1, o1 = np.zeros(12), np.zeros(n, np.uint8)
-    ok1 = ref.ref_p3p_lmeds(P(pr["bv"]), P(pr["X"]), n, 100, 3.0, K32[0], K32[1], P(T1), P(o1))
+
+    def run_ref(R):
+        R.ref_p3p_lmeds.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, f32, f32, f32, C.c_void_p, C.c_void_p]
+        R.ref_pnp.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, f32, C.c_int, C.c_int, f32, f32, f32, f32, C.c_void_p]
+        out = {"T": np.zeros(12), "outl": np.zeros(n, np.uint8)}
+        out["ok"] = R.ref_p3p_lmeds(P(pr["bv"]), P(pr["X"]), n, 100, 3.0, K32[0], K32[1], P(out["T"]), P(out["outl"]))
+        for rob, l2 in ((1, 1), (0, 0)):
+            p1, oo1 = pr["pose0"].copy(), np.zeros(n, np.uint8)
+            out[f"pnp_ok_{rob}"] = R.ref_pnp(P(pr["uv"]), P(pr["X"]), n, P(p1), 5, 5.9915, rob, l2, K32[0], K32[1], K32[2], K32[3], P(oo1))
+            out[f"pnp_pose_{rob}"], out[f"pnp_outl_{rob}"] = p1, oo1
+        return out
+    want = ref_outputs(ref, f"pose_{n}_{seed}_{of}", run_ref)
+    ok1, T1, o1 = want["ok"], want["T"], want["outl"]
     ok2, T2, o2, _ = orc_p3p(oracle, pr["bv"], pr["X"], K32)
     assert ok1 == ok2 == 1 and (o1 == o2).all() and np.abs(T1 - T2).max() < 1e-9
     for rob, l2 in ((1, 1), (0, 0)):
-        p1, oo1 = pr["pose0"].copy(), np.zeros(n, np.uint8)
-        k1 = ref.ref_pnp(P(pr["uv"]), P(pr["X"]), n, P(p1), 5, 5.9915, rob, l2, K32[0], K32[1], K32[2], K32[3], P(oo1))
+        k1, p1, oo1 = want[f"pnp_ok_{rob}"], want[f"pnp_pose_{rob}"], want[f"pnp_outl_{rob}"]
         k2, p2, oo2, _ = orc_pnp(oracle, pr["uv"], pr["X"], K32.astype(np.float64), pr["pose0"], rob, l2)
         assert k1 == k2 == 1 and (oo1 == oo2).all() and np.abs(p1 - p2).max() < 1e-9
 

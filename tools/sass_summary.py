@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Per-kernel counts of the SASS mnemonics that show what a kernel is built on (TMA, tcgen05 / TMEM, FP64 tensor cores,
+"""Per-kernel counts of the SASS mnemonics that show what a kernel is built on (TMA, wgmma, FP64 tensor cores,
 integer dot products, SWAR byte ops, population counts) from `cuobjdump -sass alvaar_b200/libalva_b200.so`.
 usage: python tools/sass_summary.py > profiles/sass_summary.txt"""
 import collections
@@ -11,7 +11,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 so = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "alvaar_b200", "libalva_b200.so")
 txt = subprocess.run(["cuobjdump", "-sass", so], capture_output=True, text=True, check=True).stdout
-PAT = [("UTMALDG", r"UTMALDG"), ("UBLKCP", r"UBLKCP"), ("UTC*MMA", r"UTC[A-Z]*MMA"), ("LDTM", r"LDTM"), ("UTCBAR", r"UTCBAR"),
+PAT = [("UTMALDG", r"UTMALDG"), ("UBLKCP", r"UBLKCP"), ("GMMA", r"[A-Z]*GMMA"),
        ("SYNCS(mbarrier)", r"SYNCS"), ("DMMA", r"DMMA"), ("IMMA", r"\bIMMA"), ("HMMA", r"HMMA"), ("IDP", r"\bIDP"), ("VABSDIFF4", r"VABSDIFF4"),
        ("VIMNMX*", r"VIMNMX"), ("POPC", r"\bPOPC"), ("LOP3", r"\bLOP3"), ("SHFL", r"\bSHFL"), ("REDUX", r"REDUX"), ("MATCH", r"\bMATCH"),
        ("DFMA", r"\bDFMA"), ("FFMA", r"\bFFMA")]
@@ -33,8 +33,8 @@ for line in txt.splitlines():
                 counts[k] += 1
 if name:
     rows.append((name, total, dict(counts)))
-print("# static SASS of", os.path.relpath(so, ROOT), "(sm_100a): instructions per kernel and the mnemonics that matter")
-print("# UTMALDG / UBLKCP = TMA (tensor / bulk copies); UTC*MMA + LDTM = tcgen05 MMA with TMEM accumulators; DMMA = FP64 tensor cores")
+print("# static SASS of", os.path.relpath(so, ROOT), "(sm_90a): instructions per kernel and the mnemonics that matter")
+print("# UTMALDG / UBLKCP = TMA (tensor / bulk copies); IGMMA / QGMMA = wgmma (int8 / fp8) with register accumulators; DMMA = FP64 tensor cores")
 cols = [k for k, _ in PAT]
 print("kernel".ljust(58), "instr".rjust(6), " ".join(c.rjust(9) for c in cols))
 for name, total, c in sorted(rows, key=lambda r: -r[1]):
