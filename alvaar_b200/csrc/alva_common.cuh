@@ -34,6 +34,8 @@ struct alva_ctx {
     uint32_t init_tab_seed = 0;
     void* knn_ws = nullptr;         // tensor-core matcher: expanded int8 operand tiles, row map (hamming_mma.cu)
     size_t knn_ws_bytes = 0;
+    void* clahe_ws = nullptr;       // alva_k_clahe's per-tile LUTs [frames][tiles_y][tiles_x][256] (clahe.cu)
+    size_t clahe_ws_bytes = 0;
     // fork / join inside one entry point (BA: the structure kernels run beside the first linearisation).  Created with the
     // context so that nothing is allocated while a caller captures `stream` into a CUDA graph.
     cudaStream_t aux_stream = nullptr;

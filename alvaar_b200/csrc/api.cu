@@ -121,6 +121,7 @@ extern "C" void alva_ctx_destroy(alva_ctx* ctx) {
     if (ctx->ba_ws) cudaFree(ctx->ba_ws);
     if (ctx->det_ws) cudaFree(ctx->det_ws);
     if (ctx->knn_ws) cudaFree(ctx->knn_ws);
+    if (ctx->clahe_ws) cudaFree(ctx->clahe_ws);
     if (ctx->p3p_tab) cudaFree(ctx->p3p_tab);
     if (ctx->init_tab) cudaFree(ctx->init_tab);
     if (ctx->aux_stream) { cudaStreamSynchronize(ctx->aux_stream); cudaStreamDestroy(ctx->aux_stream); }

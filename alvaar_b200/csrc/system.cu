@@ -12,6 +12,7 @@
 // The state machine (keypoints, map points, keyframes, motion model, the reference's gates and status codes) is
 // system_core.h; this file is its CUDA Backend -- every pixel and solver stage of a call runs on the device:
 //   pyramid      RGBA -> gray + pyramid + Scharr levels           alva_k_frontend, Scharr levels   (system.cpp:112, visual_frontend.cpp:672-698)
+//                with CLAHE on: RGBA -> raw gray -> CLAHE -> L0 -> pyrDown levels -> Scharr   alva_k_clahe, alva_k_pyrdown
 //   klt          forward-backward pyramidal LK                    alva_k_klt_fb                     (feature_tracker.cpp:5-111)
 //   detect       grid Shi-Tomasi + cornerSubPix                   alva_k_detect_grid                (feature_extractor.cpp:11-158)
 //   describe     7x7 blur + rBRIEF-256 at -1 degree               alva_k_orb_blur / _describe       (feature_extractor.cpp:160-214)
@@ -32,6 +33,8 @@
 
 int alva_scharr_levels_launch(alva_ctx* ctx, int nlev, const uint8_t* const* src, int16_t* const* dst, const int* w, const int* h,
                               int nframes);
+int alva_clahe_launch(alva_ctx* ctx, const uint8_t* src, uint8_t* dst, int w, int h, int nframes, double clip_limit, int tiles_x,
+                      int tiles_y, uint8_t* lut);
 int alva_pose_chain_launch(alva_ctx* ctx, int n, int cap, const double* bvs, const double* X, const double* uv, const double* K4,
                            float fx, float fy, uint32_t seed, double* T12, double* info, uint8_t* o1, double* uv2, double* X2,
                            int32_t* n2, double* pose7, uint8_t* o2, double* summ, double huber, double chi2);
@@ -95,6 +98,16 @@ struct CudaBackend {
     int32_t* cnt_dev = nullptr;
     double *quality_dev = nullptr, *dbl_dev = nullptr;   // dbl_dev: [A: 3 cap][B: 3 cap][C: 3 cap][small: 64]
     bool blur_valid = false;
+    // CLAHE (State::claheEnabled_ / claheContrastLimit_ / claheTileSize_, visual_frontend.cpp:16-18, 678-681).  When on, the gray
+    // frame goes to raw_dev, its equalised image is level 0: KLT and the detector read the equalised pyramid, ORB describes the
+    // raw frame (map_manager.cpp:204, 218).  Its pyramid chain differs, so it has its own graph pair, re-captured when a
+    // parameter changes; with CLAHE off nothing here is allocated and the original chain and graphs run unchanged.
+    bool clahe = false;
+    float clahe_clip = 3.f;   // a float in State (state.hpp:44)
+    int clahe_tx = 0, clahe_ty = 0, clahe_graph_launches = 0;
+    uint8_t *raw_dev = nullptr, *clahe_lut = nullptr;
+    size_t clahe_lut_bytes = 0;
+    cudaGraphExec_t clahe_graph[2] = {nullptr, nullptr};
 
     int init(int dev, int W, int H) {
         release();
@@ -144,9 +157,69 @@ struct CudaBackend {
         for (void** b : bufs) if (*b) { cudaFree(*b); *b = nullptr; }
         if (arena) { cudaFree(arena); arena = nullptr; arena_cap = 0; }
         for (int k = 0; k < 2; k++) if (pyr_graph[k]) { cudaGraphExecDestroy(pyr_graph[k]); pyr_graph[k] = nullptr; }
+        drop_clahe_graphs();
+        if (raw_dev) { cudaFree(raw_dev); raw_dev = nullptr; }
+        if (clahe_lut) { cudaFree(clahe_lut); clahe_lut = nullptr; clahe_lut_bytes = 0; }
+        clahe = false;
+        clahe_clip = 3.f;
+        clahe_tx = clahe_ty = 0;
         graphs_ok = true;
         stg.release();
         if (ctx) { alva_ctx_destroy(ctx); ctx = nullptr; }
+    }
+
+    void drop_clahe_graphs() {
+        for (int k = 0; k < 2; k++) if (clahe_graph[k]) { cudaGraphExecDestroy(clahe_graph[k]); clahe_graph[k] = nullptr; }
+    }
+    // enabled with a tx x ty grid: the buffers are allocated here, outside any capture
+    int set_clahe(bool on, float clip, int tx, int ty) {
+        if (on) {
+            if (!raw_dev) SYS_CUDA(cudaMalloc(&raw_dev, (size_t)w * h));
+            const size_t bytes = (size_t)tx * ty * 256;
+            if (bytes > clahe_lut_bytes) {
+                if (clahe_lut) { SYS_CUDA(cudaStreamSynchronize(ctx->stream)); cudaFree(clahe_lut); clahe_lut = nullptr; clahe_lut_bytes = 0; }
+                SYS_CUDA(cudaMalloc(&clahe_lut, bytes));
+                clahe_lut_bytes = bytes;
+            }
+        }
+        if (clip != clahe_clip || tx != clahe_tx || ty != clahe_ty) drop_clahe_graphs();   // the graphs bake the parameters in
+        clahe = on; clahe_clip = clip; clahe_tx = tx; clahe_ty = ty;
+        return 0;
+    }
+    uint8_t* gray_raw() { return clahe ? raw_dev : img[cur][0]; }   // what ORB describes
+
+    int clahe_launches() {
+        uint8_t** L = img[cur];
+        if (int e = alva_k_frontend(ctx, rgba_dev, w, h, 1, raw_dev, nullptr, nullptr, nullptr, 20, nullptr, nullptr, 0, 0)) return e;
+        if (int e = alva_clahe_launch(ctx, raw_dev, L[0], w, h, 1, (double)clahe_clip, clahe_tx, clahe_ty, clahe_lut)) return e;
+        for (int k = 1; k < nlev; k++)
+            if (int e = alva_k_pyrdown(ctx, L[k - 1], L[k], lw[k - 1], lh[k - 1], 1)) return e;
+        const uint8_t* srcs[4] = {L[0], L[1], L[2], L[3]};
+        return alva_scharr_levels_launch(ctx, nlev, srcs, der[cur], lw, lh, 1);
+    }
+    int pyramid_clahe() {
+        cudaStream_t st = ctx->stream;
+        if (graphs_ok && !clahe_graph[cur]) {
+            cudaGraph_t g = nullptr;
+            const long long l0 = ctx->launches;
+            bool ok = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
+            int e = 0;
+            if (ok) {
+                e = clahe_launches();
+                ok = cudaStreamEndCapture(st, &g) == cudaSuccess && e == 0 && g != nullptr;
+            }
+            if (ok) ok = cudaGraphInstantiate(&clahe_graph[cur], g, 0) == cudaSuccess;
+            if (g) cudaGraphDestroy(g);
+            clahe_graph_launches = (int)(ctx->launches - l0);
+            ctx->launches = l0;
+            if (!ok) { cudaGetLastError(); graphs_ok = false; clahe_graph[cur] = nullptr; }
+        }
+        if (clahe_graph[cur]) {
+            SYS_CUDA(cudaGraphLaunch(clahe_graph[cur], st));
+            ctx->launches += clahe_graph_launches;
+            return 0;
+        }
+        return clahe_launches();
     }
 
     int pyramid_launches() {
@@ -164,6 +237,7 @@ struct CudaBackend {
         cur ^= 1;   // VisualFrontend::preprocessImage swaps prev / cur pyramids (visual_frontend.cpp:672-698)
         blur_valid = false;
         SYS_CUDA(cudaMemcpyAsync(rgba_dev, rgba, (size_t)w * h * 4, cudaMemcpyHostToDevice, st));
+        if (clahe) return pyramid_clahe();
         if (graphs_ok && !pyr_graph[cur]) {
             cudaGraph_t g = nullptr;
             const long long l0 = ctx->launches;
@@ -212,11 +286,11 @@ struct CudaBackend {
     int describe(const float* pts, int n, uint8_t* desc, uint8_t* kept) {
         cudaStream_t st = ctx->stream;
         if (n > cap) { alva_set_error("System: %d keypoints exceed the frame capacity %d", n, cap); return ALVA_E_CAPACITY; }
-        if (!blur_valid) { if (int e = alva_k_orb_blur(ctx, img[cur][0], blur_dev, w, h, 1, 0)) return e; blur_valid = true; }
+        if (!blur_valid) { if (int e = alva_k_orb_blur(ctx, gray_raw(), blur_dev, w, h, 1, 0)) return e; blur_valid = true; }
         int32_t nn = n;
         SYS_CUDA(cudaMemcpyAsync(pri_dev, pts, (size_t)n * 8, cudaMemcpyHostToDevice, st));
         SYS_CUDA(cudaMemcpyAsync(cnt_dev + 2, &nn, 4, cudaMemcpyHostToDevice, st));
-        if (int e = alva_k_orb_describe(ctx, img[cur][0], blur_dev, w, h, 1, pri_dev, cnt_dev + 2, cap, 0, desc_dev, flag_dev, nullptr)) return e;
+        if (int e = alva_k_orb_describe(ctx, gray_raw(), blur_dev, w, h, 1, pri_dev, cnt_dev + 2, cap, 0, desc_dev, flag_dev, nullptr)) return e;
         SYS_CUDA(cudaMemcpyAsync(desc, desc_dev, (size_t)n * 32, cudaMemcpyDeviceToHost, st));
         SYS_CUDA(cudaMemcpyAsync(kept, flag_dev, n, cudaMemcpyDeviceToHost, st));
         SYS_CUDA(cudaStreamSynchronize(st));
@@ -477,7 +551,19 @@ public:
         return 0;
     }
 
-    void reset() { if (configured_) core_.reset(); }
+    void reset() { if (configured_) core_.reset(); }   // keeps the CLAHE setting (State::reset leaves it, state.cpp)
+
+    // State::claheEnabled_ / claheContrastLimit_ / claheTileSize_ and VisualFrontend's grid Size(imgWidth_ / tile, imgHeight_ / tile)
+    // (visual_frontend.cpp:16-18: a double division, truncated); configure() turns it off again (system.cpp:17)
+    int setClahe(int enabled, double clip_limit, int tile_size) {
+        if (!configured_) { alva_set_error("System: not configured"); return ALVA_E_STATE; }
+        const int tx = tile_size > 0 ? core_width() / tile_size : 0, ty = tile_size > 0 ? core_height() / tile_size : 0;
+        if (tx < 1 || ty < 1 || !(clip_limit >= 0.0)) {
+            alva_set_error("alva_system_set_clahe: tile size %d gives a %dx%d grid, clip limit %g", tile_size, tx, ty, clip_limit);
+            return ALVA_E_INVALID;
+        }
+        return be_.set_clahe(enabled != 0, (float)clip_limit, tx, ty);
+    }
 
     // returns the reference's status codes; pose16 layout as Utils::toPoseArray (src/slam/src/utils.cpp:3-27)
     int findCameraPose(const uint8_t* rgba, double t_ms, float* pose16) {
@@ -605,6 +691,8 @@ private:
         for (int r = 0; r < 3; r++) { for (int c = 0; c < 3; c++) p[4 * r + c] = (float)R[3 * r + c]; p[4 * r + 3] = 0.f; }
         p[12] = (float)T.t[0]; p[13] = (float)T.t[1]; p[14] = (float)T.t[2]; p[15] = 1.f;
     }
+    int core_width() const { return be_.w; }
+    int core_height() const { return be_.h; }
     std::vector<void*> pinned_;
     CudaBackend be_;
     alva_sys::SystemCore<CudaBackend> core_;
@@ -628,6 +716,10 @@ extern "C" int alva_system_configure(alva_system* s, int w, int h, double fx, do
                                      double k2, double p1, double p2) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
     if (!s || w < 64 || h < 64) { alva_set_error("alva_system_configure: bad argument"); return ALVA_E_INVALID; }
     return s->sys.configure(w, h, fx, fy, cx, cy, k1, k2, p1, p2);
+}
+extern "C" int alva_system_set_clahe(alva_system* s, int enabled, double clip_limit, int tile_size) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
+    if (!s) { alva_set_error("alva_system_set_clahe: null handle"); return ALVA_E_INVALID; }
+    return s->sys.setClahe(enabled, clip_limit, tile_size);
 }
 extern "C" int alva_system_reset(alva_system* s) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1); if (!s) return ALVA_E_INVALID; s->sys.reset(); return 0; }
 extern "C" int alva_system_find_camera_pose(alva_system* s, const uint8_t* rgba, float* pose16) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);

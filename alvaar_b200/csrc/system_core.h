@@ -440,8 +440,11 @@ struct MatchProblem {   // Mapper::matchToMap on flat arrays (the contract of al
 // ------------------------------------------------------------------------------------------------ the state machine
 // Backend concept (host pointers in, host pointers out; < 0 = ALVA_E_* error):
 //   int pyramid(const uint8_t* rgba)                       gray + pyramid + Scharr levels of the new frame; previous <- current
-//   int detect(const float* cur, int ncur, std::vector<float>& fresh)    grid detector on the current image (adaptive quality kept)
-//   int describe(const float* pts, int n, uint8_t* desc, uint8_t* kept)  ORB at the given points of the current image
+//                                                          (with CLAHE on, a backend matter: the pyramid is built on the equalised
+//                                                          gray frame, visual_frontend.cpp:672-698)
+//   int detect(const float* cur, int ncur, std::vector<float>& fresh)    grid detector on the current (equalised) image (adaptive quality kept)
+//   int describe(const float* pts, int n, uint8_t* desc, uint8_t* kept)  ORB at the given points of the current RAW gray image
+//                                                                        (map_manager.cpp:204, 218)
 //   int klt(const float* pts, float* priors, int n, int levels, uint8_t* good)   forward-backward KLT previous -> current
 //   int essential(const double* bv1, const double* bv2, int n, float fx, float fy, double* Rt12, uint8_t* outlier)  -> 1 / 0
 //   int p3p(const double* bv, const double* X, int n, float fx, float fy, double* T12, uint8_t* outlier)            -> 1 / 0

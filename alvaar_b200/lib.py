@@ -59,6 +59,7 @@ _OPTIONAL = {
     "alva_k_hamming_knn2_batch": [_vp, _vp, _vp, _i32, _i32, _vp, _i32, _vp],
     "alva_h_frontend": [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _i32],
     "alva_k_scharr": [_vp, _vp, _vp, _i32, _i32, _i32],
+    "alva_k_clahe": [_vp, _vp, _vp, _i32, _i32, _i32, C.c_double, _i32, _i32],
     "alva_k_detect_grid": [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _i32],
     "alva_k_corner_subpix": [_vp, _vp, _i32, _i32, _i32, _vp, _vp, _i32],
     "alva_k_match_to_map": [_vp, _i32, _i32, _i32, C.c_double, C.c_double, C.c_double, C.c_double, _vp, _i32, _vp, _vp, _i32, _i32, _vp,
@@ -174,6 +175,10 @@ class Context:
 
     def scharr(self, gray, deriv, w, h, nframes=1):
         self._chk(self.L.alva_k_scharr(self.h, _ptr(gray), _ptr(deriv), w, h, nframes))
+
+    def clahe(self, src, dst, w, h, nframes, clip_limit, tiles_x, tiles_y):
+        """cv::createCLAHE(clip_limit, (tiles_x, tiles_y))->apply on [nframes][h][w] uint8 frames; dst may be src"""
+        self._chk(self.L.alva_k_clahe(self.h, _ptr(src), _ptr(dst), w, h, nframes, float(clip_limit), tiles_x, tiles_y))
 
     @staticmethod
     def _ptr_table(levels):

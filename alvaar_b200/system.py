@@ -17,6 +17,7 @@ def _bind():
     L.alva_system_create.argtypes = [_i32]
     L.alva_system_destroy.argtypes = [_vp]
     L.alva_system_reset.argtypes = [_vp]
+    L.alva_system_set_clahe.argtypes = [_vp, _i32, _f64, _i32]
     L.alva_system_num_matched.argtypes = [_vp]
     L.alva_system_configure.argtypes = [_vp, _i32, _i32] + [_f64] * 8
     L.alva_system_find_camera_pose.argtypes = [_vp, _vp, _vp]
@@ -119,3 +120,12 @@ class System:
 
     def reset(self):
         self.L.alva_system_reset(self.h)
+
+    def set_clahe(self, enabled=True, clip_limit=3.0, tile_size=50):
+        """CLAHE on the gray frame before the KLT pyramid and the detector (the reference's State::claheEnabled_,
+        claheContrastLimit_, claheTileSize_; its ACCURATE preset turns it on with these defaults).  The grid is
+        (width // tile_size) x (height // tile_size); ORB descriptors keep reading the raw gray frame.  Applies from the next
+        frame, survives reset(); a new System starts with it off."""
+        rc = self.L.alva_system_set_clahe(self.h, 1 if enabled else 0, float(clip_limit), int(tile_size))
+        if rc != 0:
+            raise AlvaError(f"alva_system_set_clahe -> {rc}: {self.L.alva_last_error().decode()}")

@@ -77,6 +77,12 @@ int alva_k_pyrdown(alva_ctx*, const uint8_t* src, uint8_t* dst, int w, int h, in
  * image with a CONSTANT 0 border of the window size; that padding is a view concern of its Mat, not stored here.) */
 int alva_k_scharr(alva_ctx*, const uint8_t* gray, int16_t* deriv, int w, int h, int nframes);
 
+/* CLAHE: cv::createCLAHE(clip_limit, Size(tiles_x, tiles_y))->apply(src, dst), 8-bit, bit-exact (the reference's optional
+ * pre-processing before the KLT pyramid, visual_frontend.cpp:672-698 -> opencv imgproc/src/clahe.cpp:142-313, 349-429).
+ * src / dst: [nframes][h][w] u8 device buffers; dst may equal src.  clip_limit 0 = no clipping.  ALVA_E_INVALID for
+ * tiles < 1, tiles > the image size on either axis, or a negative / NaN clip_limit. */
+int alva_k_clahe(alva_ctx*, const uint8_t* src, uint8_t* dst, int w, int h, int nframes, double clip_limit, int tiles_x, int tiles_y);
+
 /* cv::FAST(gray, thr, nms=true, TYPE_9_16) on each frame (opencv features2d/src/fast.cpp:496).
  * keys[f*cap + i]: packed corner keys; counts[f] = true number found (may exceed cap: then only cap
  * are stored and the call returns ALVA_E_CAPACITY after completing).  sorted != 0: row-major order. */
@@ -378,6 +384,12 @@ void alva_system_destroy(alva_system*);
 int  alva_system_configure(alva_system*, int w, int h, double fx, double fy, double cx, double cy,
                            double k1, double k2, double p1, double p2);
 int  alva_system_reset(alva_system*);
+/* CLAHE on the gray frame before the KLT pyramid and the detector: State::claheEnabled_ / claheContrastLimit_ / claheTileSize_
+ * (state.hpp:43-45) with VisualFrontend's grid, Size(w / tile_size, h / tile_size) (visual_frontend.cpp:16-18).  ORB descriptors
+ * stay on the raw gray frame (map_manager.cpp:204, 218).  Off by default; configure turns it off again (system.cpp:17), reset keeps
+ * it; it applies from the next frame.  ALVA_E_STATE before configure; ALVA_E_INVALID for an empty grid (tile_size > w or h, or
+ * < 1) or, when enabling, a negative / NaN clip_limit. */
+int  alva_system_set_clahe(alva_system*, int enabled, double clip_limit, int tile_size);
 int  alva_system_find_camera_pose(alva_system*, const uint8_t* rgba, float* pose16);
 /* the same with the frame's time stamp (milliseconds) supplied by the caller instead of read from the system clock
  * (system.cpp:114): deterministic replays, and hosts that deliver frames faster than real time (two frames inside one
