@@ -22,7 +22,9 @@
 //   match_to_map local map -> keyframe matching                   alva_k_match_to_map               (mapper.cpp:354-587)
 //   ba_local     local bundle adjustment, both solves + flags     alva_k_ba_local                   (optimizer.cpp:251-359)
 // There is no CPU fallback: configure() fails without an sm_90 (H100) device.  Lens distortion: the JS shim always passes zeros
-// (system.js:84-141); non-zero coefficients are rejected rather than silently ignored.
+// (system.js:84-141) and configure() rejects non-zero coefficients; setDistortion() (alva_system_set_distortion) sets them on a
+// configured System.  With distortion on, klt and detect undistort the points they return with alva_k_undistort_points on the
+// device, in the same download (camera.cu, camera_model.h).
 #include "alva_common.cuh"
 #include "../../include/alva_b200.h"
 #include "system_core.h"
@@ -35,6 +37,8 @@ int alva_scharr_levels_launch(alva_ctx* ctx, int nlev, const uint8_t* const* src
                               int nframes);
 int alva_clahe_launch(alva_ctx* ctx, const uint8_t* src, uint8_t* dst, int w, int h, int nframes, double clip_limit, int tiles_x,
                       int tiles_y, uint8_t* lut);
+int alva_undistort_points_launch(alva_ctx* ctx, const float* px, const int32_t* counts, int nframes, int cap, const double* K4,
+                                 const double* D4, float* unpx);
 int alva_pose_chain_launch(alva_ctx* ctx, int n, int cap, const double* bvs, const double* X, const double* uv, const double* K4,
                            float fx, float fy, uint32_t seed, double* T12, double* info, uint8_t* o1, double* uv2, double* X2,
                            int32_t* n2, double* pose7, uint8_t* o2, double* summ, double huber, double chi2);
@@ -108,6 +112,12 @@ struct CudaBackend {
     uint8_t *raw_dev = nullptr, *clahe_lut = nullptr;
     size_t clahe_lut_bytes = 0;
     cudaGraphExec_t clahe_graph[2] = {nullptr, nullptr};
+    // lens distortion (CameraCalibration::D_): when on, klt() and detect() also return the undistorted positions of their points
+    // (unpx()); with it off nothing here is allocated or launched
+    bool has_dist = false;
+    double K4[4] = {0, 0, 0, 0}, D4[4] = {0, 0, 0, 0};
+    float* unpx_dev = nullptr;
+    std::vector<float> unpx_host;
 
     int init(int dev, int W, int H) {
         release();
@@ -160,6 +170,8 @@ struct CudaBackend {
         drop_clahe_graphs();
         if (raw_dev) { cudaFree(raw_dev); raw_dev = nullptr; }
         if (clahe_lut) { cudaFree(clahe_lut); clahe_lut = nullptr; clahe_lut_bytes = 0; }
+        if (unpx_dev) { cudaFree(unpx_dev); unpx_dev = nullptr; }
+        has_dist = false;
         clahe = false;
         clahe_clip = 3.f;
         clahe_tx = clahe_ty = 0;
@@ -187,6 +199,15 @@ struct CudaBackend {
         return 0;
     }
     uint8_t* gray_raw() { return clahe ? raw_dev : img[cur][0]; }   // what ORB describes
+
+    int set_distortion(const double* d) {
+        has_dist = d[0] != 0.0 || d[1] != 0.0 || d[2] != 0.0 || d[3] != 0.0;
+        for (int i = 0; i < 4; i++) D4[i] = d[i];
+        K4[0] = fx; K4[1] = fy; K4[2] = cx; K4[3] = cy;
+        if (has_dist && !unpx_dev) SYS_CUDA(cudaMalloc(&unpx_dev, (size_t)cap * 8));
+        return 0;
+    }
+    const float* unpx() const { return has_dist ? unpx_host.data() : nullptr; }
 
     int clahe_launches() {
         uint8_t** L = img[cur];
@@ -269,6 +290,8 @@ struct CudaBackend {
         const int32_t roi[4] = {20, 20, w - 40, h - 40};   // CameraCalibration(..., imgBorder 20): roi_rect_ (camera_calibration.cpp:21)
         if (int e = alva_k_detect_grid(ctx, img[cur][0], w, h, 1, 40, pts_dev, cnt_dev + 1, cap, roi, quality_dev, pri_dev, nullptr, cnt_dev, cap))
             return e;
+        if (has_dist)   // Frame::computeKeypoint's undistortImagePoint of every new keypoint (frame.cpp:101-109)
+            if (int e = alva_undistort_points_launch(ctx, pri_dev, cnt_dev, 1, cap, K4, D4, unpx_dev)) return e;
         int32_t n = 0;
         SYS_CUDA(cudaMemcpyAsync(&n, cnt_dev, 4, cudaMemcpyDeviceToHost, st));
         SYS_CUDA(cudaStreamSynchronize(st));
@@ -276,6 +299,10 @@ struct CudaBackend {
         fresh.resize((size_t)2 * n);
         if (n) {
             SYS_CUDA(cudaMemcpyAsync(fresh.data(), pri_dev, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
+            if (has_dist) {
+                unpx_host.resize((size_t)2 * n);
+                SYS_CUDA(cudaMemcpyAsync(unpx_host.data(), unpx_dev, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
+            }
             SYS_CUDA(cudaStreamSynchronize(st));
         }
         return 0;
@@ -308,16 +335,20 @@ struct CudaBackend {
         float* dq = stg.take<float>((size_t)2 * n, &hq);
         const size_t q_off = (uint8_t*)dq - stg.d, up_end = stg.off;
         uint8_t* dg = stg.take<uint8_t>(n, &hg);
+        float *hu = nullptr, *du = has_dist ? stg.take<float>((size_t)2 * n, &hu) : nullptr;   // the tracked points, undistorted
         memcpy(hp, pts, (size_t)n * 8);
         memcpy(hq, priors, (size_t)n * 8);
         SYS_CUDA(cudaMemcpyAsync(stg.d, stg.h, up_end, cudaMemcpyHostToDevice, st));
         const int prev = cur ^ 1;
         if (int e = alva_k_klt_fb(ctx, img[prev], der[prev], img[cur], der[cur], w, h, 1, nlev - 1, levels, 9, 30.0f, 0.5f, dp, dq, nullptr, n, dg))
             return e;
+        if (has_dist)   // Frame::computeKeypoint's undistortImagePoint of every tracked keypoint (frame.cpp:101-109)
+            if (int e = alva_undistort_points_launch(ctx, dq, nullptr, 1, n, K4, D4, du)) return e;
         SYS_CUDA(cudaMemcpyAsync(stg.h + q_off, stg.d + q_off, stg.off - q_off, cudaMemcpyDeviceToHost, st));
         SYS_CUDA(cudaStreamSynchronize(st));
         memcpy(priors, hq, (size_t)n * 8);
         memcpy(good, hg, n);
+        if (has_dist) unpx_host.assign(hu, hu + 2 * (size_t)n);
         return 0;
     }
 
@@ -502,8 +533,8 @@ struct CudaBackend {
         int32_t* lm = arena_put(m.local_mp.data(), n_local);
         int32_t* out = arena_take<int32_t>(n_kp);
         int32_t* nm = arena_take<int32_t>(4);
-        if (int e = alva_k_match_to_map(ctx, w, h, 40, fx, fy, cx, cy, Tc, (int)n_kp, kpmp, kppx, m.nkp3d, (int)(n_kf ? n_kf : 1), kfT, (int)n_mp, wpt, is3,
-                                        os, ok, op, ds, dd, (int)n_local, lm, 2.0f, 0.2f, out, nullptr, nm))
+        if (int e = alva_k_match_to_map_dist(ctx, w, h, 40, fx, fy, cx, cy, Tc, (int)n_kp, kpmp, kppx, m.nkp3d, (int)(n_kf ? n_kf : 1), kfT, (int)n_mp,
+                                             wpt, is3, os, ok, op, ds, dd, (int)n_local, lm, 2.0f, 0.2f, out, nullptr, nm, m.has_dist ? m.dist : nullptr))
             return e;
         std::vector<int32_t> host(n_kp);
         SYS_CUDA(cudaMemcpyAsync(host.data(), out, n_kp * 4, cudaMemcpyDeviceToHost, st));
@@ -541,7 +572,8 @@ public:
                   double p2) {
         configured_ = false;
         if (k1 != 0. || k2 != 0. || p1 != 0. || p2 != 0.) {
-            alva_set_error("System::configure: non-zero lens distortion is not supported (the reference's shim always passes zeros)");
+            alva_set_error("System::configure: non-zero lens distortion is not accepted here (the reference's shim always passes zeros); "
+                           "configure with zeros, then set the coefficients with alva_system_set_distortion");
             return ALVA_E_INVALID;
         }
         if (int e = be_.init(device_, imageWidth, imageHeight)) return e;
@@ -551,7 +583,19 @@ public:
         return 0;
     }
 
-    void reset() { if (configured_) core_.reset(); }   // keeps the CLAHE setting (State::reset leaves it, state.cpp)
+    void reset() { if (configured_) core_.reset(); }   // keeps the CLAHE setting (State::reset leaves it, state.cpp) and the lens model
+
+    // CameraCalibration's k1 k2 p1 p2 (camera_calibration.cpp:3-24): the tracker and the map restart under the new model;
+    // configure() sets them back to zero
+    int setDistortion(double k1, double k2, double p1, double p2) {
+        if (!configured_) { alva_set_error("System: not configured"); return ALVA_E_STATE; }
+        const double d[4] = {k1, k2, p1, p2};
+        for (double v : d)
+            if (!std::isfinite(v)) { alva_set_error("alva_system_set_distortion: non-finite coefficient"); return ALVA_E_INVALID; }
+        if (int e = be_.set_distortion(d)) return e;
+        core_.setDistortion(d);
+        return 0;
+    }
 
     // State::claheEnabled_ / claheContrastLimit_ / claheTileSize_ and VisualFrontend's grid Size(imgWidth_ / tile, imgHeight_ / tile)
     // (visual_frontend.cpp:16-18: a double division, truncated); configure() turns it off again (system.cpp:17)
@@ -720,6 +764,10 @@ extern "C" int alva_system_configure(alva_system* s, int w, int h, double fx, do
 extern "C" int alva_system_set_clahe(alva_system* s, int enabled, double clip_limit, int tile_size) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
     if (!s) { alva_set_error("alva_system_set_clahe: null handle"); return ALVA_E_INVALID; }
     return s->sys.setClahe(enabled, clip_limit, tile_size);
+}
+extern "C" int alva_system_set_distortion(alva_system* s, double k1, double k2, double p1, double p2) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
+    if (!s) { alva_set_error("alva_system_set_distortion: null handle"); return ALVA_E_INVALID; }
+    return s->sys.setDistortion(k1, k2, p1, p2);
 }
 extern "C" int alva_system_reset(alva_system* s) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1); if (!s) return ALVA_E_INVALID; s->sys.reset(); return 0; }
 extern "C" int alva_system_find_camera_pose(alva_system* s, const uint8_t* rgba, float* pose16) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);

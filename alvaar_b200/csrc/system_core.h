@@ -39,6 +39,7 @@
 #include <unordered_set>
 #include <vector>
 #include <random>
+#include "camera_model.h"
 
 namespace alva_sys {
 
@@ -148,7 +149,16 @@ struct Se3 {
 struct Camera {
     double fx = 1, fy = 1, cx = 0, cy = 0;
     int w = 0, h = 0;
-    // CameraCalibration::undistortImagePoint with the zero distortion the shim always passes: cv::undistortPoints(..., K, D, K)
+    // lens distortion k1 k2 p1 p2 (CameraCalibration::D_); has_dist = any of them non-zero.  Without it the two functions that
+    // apply it below take their pinhole forms, which give the same bits as the radial-tangential model with zero coefficients.
+    double dist[4] = {0, 0, 0, 0};
+    bool has_dist = false;
+    void setDistortion(const double* d) {
+        has_dist = false;
+        for (int i = 0; i < 4; i++) { dist[i] = d[i]; has_dist = has_dist || d[i] != 0.0; }
+    }
+    void K4(double* k) const { k[0] = fx; k[1] = fy; k[2] = cx; k[3] = cy; }
+    // CameraCalibration::undistortImagePoint: cv::undistortPoints(..., K, D, K) (camera_model.h); with zero distortion it
     // evaluates fx * ((u - cx) * (1 / fx)) + cx in double and rounds to float (calib3d/src/undistort.dispatch.cpp)
     double ifx = 1, ify = 1, k00 = 1, k02 = 0, k11 = 1, k12 = 0, k22 = 1;   // loop invariants of the two functions below
     void prepare() {
@@ -157,6 +167,14 @@ struct Camera {
         k00 = fy * id; k02 = (-(cx * fy)) * id; k11 = fx * id; k12 = (-(fx * cy)) * id; k22 = (fx * fy) * id;
     }
     void undistort(float u, float v, float& ux, float& uy) const {
+        if (has_dist) {
+            double k[4];
+            float o[2];
+            K4(k);
+            alva_cam::undistort_point(k, dist, u, v, o);
+            ux = o[0]; uy = o[1];
+            return;
+        }
         const double x = ((double)u - cx) * ifx, y = ((double)v - cy) * ify;
         ux = (float)(fx * x + cx); uy = (float)(fy * y + cy);
     }
@@ -180,6 +198,14 @@ struct Camera {
         u = (float)(fx * (p[0] * iz) + cx); v = (float)(fy * (p[1] * iz) + cy);
     }
     void projCamToImageDist(const double* p, float& u, float& v) const {   // :34-55: cv::projectPoints on a FLOAT point
+        if (has_dist) {
+            double k[4];
+            float o[2];
+            K4(k);
+            alva_cam::project_dist(k, dist, p, o);
+            u = o[0]; v = o[1];
+            return;
+        }
         const double iz = 1. / p[2];
         const double x = (double)(float)(p[0] * iz), y = (double)(float)(p[1] * iz);
         u = (float)(x * fx + cx); v = (float)(y * fy + cy);
@@ -228,9 +254,11 @@ struct Frame {
     }
     void setTwc(const Se3& T) { Twc = T; Tcw = T.inverse(); }
     int cellIdx(float x, float y) const { return (int)floor(y / (float)cell) * ncw + (int)floor(x / (float)cell); }
-    void compute(float x, float y, Keypoint& k) const {
+    // un: the undistorted position when the backend computed it (the same model on the device), else NULL
+    void compute(float x, float y, Keypoint& k, const float* un = nullptr) const {
         k.px = x; k.py = y;
-        cam->undistort(x, y, k.ux, k.uy);
+        if (un) { k.ux = un[0]; k.uy = un[1]; }
+        else cam->undistort(x, y, k.ux, k.uy);
         cam->bearing(k.ux, k.uy, k.bv);
     }
     void gridAdd(const Keypoint& k) {
@@ -253,19 +281,19 @@ struct Frame {
         n++;
         if (k.is3d) n3d++; else n2d++;
     }
-    void add(float x, float y, int id, const uint8_t* desc) {
+    void add(float x, float y, int id, const uint8_t* desc, const float* un = nullptr) {
         Keypoint k;
         k.id = id;
-        compute(x, y, k);
+        compute(x, y, k, un);
         if (desc) { k.has_desc = true; memcpy(k.desc, desc, 32); }
         add(k);
     }
-    void update(int id, float x, float y) {
+    void update(int id, float x, float y, const float* un = nullptr) {
         auto it = kps.find(id);
         if (it == kps.end()) return;
         Keypoint& k = it->second;   // same effect as the reference's copy / recompute / updateKeypointInGrid / assign
-        if (cellIdx(k.px, k.py) != cellIdx(x, y)) { gridRemove(k); compute(x, y, k); gridAdd(k); }
-        else compute(x, y, k);
+        if (cellIdx(k.px, k.py) != cellIdx(x, y)) { gridRemove(k); compute(x, y, k, un); gridAdd(k); }
+        else compute(x, y, k, un);
     }
     void remove(int id) {
         auto it = kps.find(id);
@@ -408,6 +436,12 @@ struct MotionModel {   // visual_frontend.hpp:17-56
 template <class B, class = void> struct BackendHasPoseChain : std::false_type {};
 template <class B> struct BackendHasPoseChain<B, std::void_t<decltype(std::declval<B&>().has_pose_chain())>> : std::true_type {};
 
+// a Backend may undistort the points its klt() and detect() return (the CUDA backend does it on the device, in the same
+// download): unpx() then gives their undistorted positions [n][2] until its next call, or NULL when it did not compute them.
+// Backends without it (the CPU oracle backend) leave it to Camera::undistort -- the same arithmetic (camera_model.h).
+template <class B, class = void> struct BackendHasUnpx : std::false_type {};
+template <class B> struct BackendHasUnpx<B, std::void_t<decltype(std::declval<B&>().unpx())>> : std::true_type {};
+
 // ------------------------------------------------------------------------------------------------ flat problems handed to a Backend
 struct BaProblem {   // the layout of alva_k_ba_local
     int nkf = 0, nlm = 0, nobs = 0;
@@ -435,6 +469,8 @@ struct MatchProblem {   // Mapper::matchToMap on flat arrays (the contract of al
     std::vector<int32_t> desc_start, desc_kfid;
     std::vector<uint8_t> desc;
     std::vector<int32_t> local_mp;      // table indices of the local map, in the set's iteration order
+    bool has_dist = false;              // lens distortion of the projections (Camera::dist)
+    double dist[4] = {0, 0, 0, 0};
 };
 
 // ------------------------------------------------------------------------------------------------ the state machine
@@ -452,6 +488,7 @@ struct MatchProblem {   // Mapper::matchToMap on flat arrays (the contract of al
 //   int triangulate(const double* Tlr7, const double* bvl, const double* bvr, int n, double* out)
 //   bool has_ba_local(); int ba_local(BaProblem& io, int32_t* flags)         Optimizer::localBA's numerical body (two solves + flags)
 //   bool has_match_to_map(); int match_to_map(const MatchProblem&, std::vector<int>& kp_match)   Mapper::matchToMap
+//   optional: const float* unpx()                          see BackendHasUnpx
 template <class Backend>
 class SystemCore {
 public:
@@ -460,9 +497,17 @@ public:
     void configure(int w, int h, double fx, double fy, double cx, double cy) {
         cam.w = w; cam.h = h; cam.fx = fx; cam.fy = fy; cam.cx = cx; cam.cy = cy;
         cam.prepare();
+        const double zero[4] = {0, 0, 0, 0};
+        cam.setDistortion(zero);
         cell = 40;                                                        // State(w, h, 40) (system.cpp:15)
         max_kps = (int)(ceil((double)w / cell) * ceil((double)h / cell));   // state.cpp:3-12
         cur.init(&cam, cell);                                             // Frame(calibration, State::frameMaxCellSize_ = 40)
+        reset();
+    }
+
+    // the lens model of every later frame; the map and the tracked keypoints were made under the previous one: reset
+    void setDistortion(const double* d) {
+        cam.setDistortion(d);
         reset();
     }
 
@@ -688,6 +733,9 @@ private:
             std::vector<float> fresh;
             if ((err = B.detect(pts.data(), (int)kps.size(), fresh)) < 0) return;
             err = 0;
+            const float* un = backendUnpx();
+            std::vector<float> fresh_un;
+            if (un) fresh_un.assign(un, un + fresh.size());   // describe() below may reuse the backend's buffer
             const int nn = (int)fresh.size() / 2;
             if (nn > 0) {
                 std::vector<uint8_t> desc(32 * (size_t)nn), kept(nn);
@@ -695,7 +743,7 @@ private:
                 err = 0;
                 for (int i = 0; i < nn; i++) {   // addKeypointsToFrame + addMapPoint (map_manager.cpp:152-191, 255-330)
                     const uint8_t* d = kept[i] ? &desc[32 * (size_t)i] : nullptr;
-                    cur.add(fresh[2 * i], fresh[2 * i + 1], n_mp_ids, d);
+                    cur.add(fresh[2 * i], fresh[2 * i + 1], n_mp_ids, d, un ? &fresh_un[2 * (size_t)i] : nullptr);
                     MapPoint mp;
                     mp.id = n_mp_ids; mp.kfid = n_kf_ids; mp.observed = true;
                     mp.obs.insert(n_kf_ids);
@@ -807,6 +855,8 @@ private:
     void buildMatchProblem(const Frame& frame, MatchProblem& m) {
         frame.Twc.to7(m.Twc_cur);
         m.nkp3d = frame.n3d;
+        m.has_dist = cam.has_dist;
+        for (int i = 0; i < 4; i++) m.dist[i] = cam.dist[i];
         // the frame's keypoints cell by cell, each cell in its insertion order (what Frame::getSurroundingKeypoints walks)
         std::unordered_map<int, int> mp_index;
         auto add_mp = [&](int id) -> int {
@@ -1160,9 +1210,10 @@ private:
             std::vector<uint8_t> good(n3);
             if ((err = B.klt(kps3.data(), pri3.data(), (int)n3, 1, good.data())) < 0) return;
             err = 0;
+            const float* un = backendUnpx();
             size_t ngood = 0;
             for (size_t i = 0; i < n3; i++) {
-                if (good[i]) { cur.update(ids3[i], pri3[2 * i], pri3[2 * i + 1]); ngood++; }
+                if (good[i]) { cur.update(ids3[i], pri3[2 * i], pri3[2 * i + 1], un ? un + 2 * i : nullptr); ngood++; }
                 else { ids.push_back(ids3[i]); kps.push_back(kps3[2 * i]); kps.push_back(kps3[2 * i + 1]); pri.push_back(pri3[2 * i]); pri.push_back(pri3[2 * i + 1]); }
             }
             if (ngood < 0.33 * n3) { p3p_req = true; pri = kps; }
@@ -1172,11 +1223,18 @@ private:
             std::vector<uint8_t> good(n);
             if ((err = B.klt(kps.data(), pri.data(), (int)n, 3, good.data())) < 0) return;   // State::kltPyramidLevels_
             err = 0;
+            const float* un = backendUnpx();
             for (size_t i = 0; i < n; i++) {
-                if (good[i]) cur.update(ids[i], pri[2 * i], pri[2 * i + 1]);
+                if (good[i]) cur.update(ids[i], pri[2 * i], pri[2 * i + 1], un ? un + 2 * i : nullptr);
                 else removeObsFromCurr(ids[i]);
             }
         }
+    }
+
+    // the undistorted positions of the points the last klt() / detect() returned, when the backend computed them
+    const float* backendUnpx() {
+        if constexpr (BackendHasUnpx<Backend>::value) if (cam.has_dist) return B.unpx();
+        return nullptr;
     }
 
     void resetFrame() {   // visual_frontend.cpp:700-716

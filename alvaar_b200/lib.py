@@ -64,6 +64,10 @@ _OPTIONAL = {
     "alva_k_corner_subpix": [_vp, _vp, _i32, _i32, _i32, _vp, _vp, _i32],
     "alva_k_match_to_map": [_vp, _i32, _i32, _i32, C.c_double, C.c_double, C.c_double, C.c_double, _vp, _i32, _vp, _vp, _i32, _i32, _vp,
                             _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, C.c_float, C.c_float, _vp, _vp, _vp],
+    "alva_k_match_to_map_dist": [_vp, _i32, _i32, _i32, C.c_double, C.c_double, C.c_double, C.c_double, _vp, _i32, _vp, _vp, _i32, _i32,
+                                 _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, C.c_float, C.c_float, _vp, _vp, _vp, _vp],
+    "alva_k_undistort_points": [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp],
+    "alva_k_project_points": [_vp, _vp, _i32, _vp, _vp, _vp],
     "alva_k_p3p_lmeds": [_vp, _i32, _i32, _vp, _vp, _vp, _i32, C.c_float, C.c_float, C.c_float, C.c_uint32, _vp, _vp, _vp],
     "alva_k_pnp": [_vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, C.c_double, C.c_double, _i32, _i32, _i32, _vp, _vp],
     "alva_k_essential_5pt": [_vp, _i32, _i32, _vp, _vp, _vp, _i32, C.c_float, _i32, C.c_float, C.c_float, C.c_uint32, _vp, _vp, _vp],
@@ -102,6 +106,11 @@ def _ptr(t):
     if t is None:
         return None
     return C.c_void_p(t.data_ptr())
+
+
+def _f64x4(v):
+    """four host doubles (intrinsics or distortion coefficients)"""
+    return (C.c_double * 4)(*[float(x) for x in v])
 
 
 class Context:
@@ -210,13 +219,27 @@ class Context:
         self._chk(self.L.alva_k_corner_subpix(self.h, _ptr(gray), w, h, nframes, _ptr(pts), _ptr(counts), cap))
 
     def match_to_map(self, w, h, cell, K, Twc_cur, kp_mp, kp_px, nkp3d, kf_Twc, mp_wpt, mp_is3d, obs_start, obs_kf, obs_px,
-                     desc_start, desc, local_mp, kp_match, kp_dist, n_match, max_proj_err=2.0, dist_ratio=0.2):
-        """Mapper::matchToMap on flat device arrays -- see alva_k_match_to_map."""
-        self._chk(self.L.alva_k_match_to_map(self.h, w, h, cell, K[0], K[1], K[2], K[3], _ptr(Twc_cur), kp_mp.numel(), _ptr(kp_mp),
-                                             _ptr(kp_px), nkp3d, kf_Twc.shape[0], _ptr(kf_Twc), mp_wpt.shape[0], _ptr(mp_wpt),
-                                             _ptr(mp_is3d), _ptr(obs_start), _ptr(obs_kf), _ptr(obs_px), _ptr(desc_start),
-                                             _ptr(desc), local_mp.numel(), _ptr(local_mp), max_proj_err, dist_ratio,
-                                             _ptr(kp_match), _ptr(kp_dist), _ptr(n_match)))
+                     desc_start, desc, local_mp, kp_match, kp_dist, n_match, max_proj_err=2.0, dist_ratio=0.2, dist=None):
+        """Mapper::matchToMap on flat device arrays -- see alva_k_match_to_map; dist = (k1, k2, p1, p2): the lens-distorted
+        projections of alva_k_match_to_map_dist."""
+        args = (self.h, w, h, cell, K[0], K[1], K[2], K[3], _ptr(Twc_cur), kp_mp.numel(), _ptr(kp_mp), _ptr(kp_px), nkp3d,
+                kf_Twc.shape[0], _ptr(kf_Twc), mp_wpt.shape[0], _ptr(mp_wpt), _ptr(mp_is3d), _ptr(obs_start), _ptr(obs_kf),
+                _ptr(obs_px), _ptr(desc_start), _ptr(desc), local_mp.numel(), _ptr(local_mp), max_proj_err, dist_ratio,
+                _ptr(kp_match), _ptr(kp_dist), _ptr(n_match))
+        if dist is None:
+            self._chk(self.L.alva_k_match_to_map(*args))
+        else:
+            self._chk(self.L.alva_k_match_to_map_dist(*args, _f64x4(dist)))
+
+    def undistort_points(self, px, counts, nframes, cap, K, dist, unpx):
+        """cv::undistortPoints(px, unpx, K, D, K) for px [nframes][cap][2] float32 (counts: int32 [nframes] device tensor or None
+        = cap points per frame) -- see alva_k_undistort_points.  K = (fx, fy, cx, cy), dist = (k1, k2, p1, p2)."""
+        self._chk(self.L.alva_k_undistort_points(self.h, _ptr(px), _ptr(counts), nframes, cap, _f64x4(K), _f64x4(dist), _ptr(unpx)))
+
+    def project_points(self, Xc, n, K, dist, uv):
+        """CameraCalibration::projectCamToImageDist of n camera-frame points Xc [n][3] float64 into uv [n][2] float32 -- see
+        alva_k_project_points."""
+        self._chk(self.L.alva_k_project_points(self.h, _ptr(Xc), n, _f64x4(K), _f64x4(dist), _ptr(uv)))
 
     def p3p_lmeds(self, nprob, cap, bvs, wpts, counts, Twc_out, outlier, info=None, max_iter=100, err_px=3.0, fx=1.0, fy=1.0,
                   seed=12345):

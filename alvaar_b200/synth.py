@@ -4,7 +4,8 @@
             contrast-normalised to mean 128 / std 60 and clipped -- about 15 k FAST-9 (thr 20, NMS) corners per
             1280x720 view, so 1000 features/frame is always reachable.
 * frames  : a pinhole camera on a smooth seeded SE(3) trajectory (about 3 px/frame lateral motion, +-0.2 deg/frame
-            rotation) looking at the texture plane z = 4; bilinear sampling; RGBA with R = G = B, A = 255.
+            rotation) looking at the texture plane z = 4; bilinear sampling; RGBA with R = G = B, A = 255.  Optionally
+            through OpenCV's radial-tangential lens (k1, k2, p1, p2).
 * descriptors / BA problems for the matcher and bundle-adjustment stages.
 Pure numpy (+ scipy.ndimage for the blur); nothing here is on the product path.
 """
@@ -63,14 +64,35 @@ def trajectory(nframes, w, h, seed=99, plane_z=4.0):
     return poses
 
 
-def render_gray(tex, pose, w, h, plane_z=4.0, tex_scale=None):
-    """Bilinear render of the texture plane z = plane_z seen from pose (R_wc, t_wc)."""
+def undistort_normalised(xd, yd, dist, tol=1e-12, max_iter=500):
+    """The normalised point (x, y) that OpenCV's radial-tangential model (k1, k2, p1, p2) maps to (xd, yd): fixed-point
+    iteration run to convergence (scene generation, not the reference's 5-iteration cv::undistortPoints)."""
+    k1, k2, p1, p2 = dist
+    x, y = xd.copy(), yd.copy()
+    for _ in range(max_iter):
+        r2 = x * x + y * y
+        radial = 1 + k1 * r2 + k2 * r2 * r2
+        nx = (xd - (2 * p1 * x * y + p2 * (r2 + 2 * x * x))) / radial
+        ny = (yd - (p1 * (r2 + 2 * y * y) + 2 * p2 * x * y)) / radial
+        done = max(np.abs(nx - x).max(), np.abs(ny - y).max()) < tol
+        x, y = nx, ny
+        if done:
+            return x, y
+    raise ValueError(f"lens model {dist} does not invert over this image")
+
+
+def render_gray(tex, pose, w, h, plane_z=4.0, tex_scale=None, dist=None):
+    """Bilinear render of the texture plane z = plane_z seen from pose (R_wc, t_wc); dist = (k1, k2, p1, p2): through that lens."""
     fx, fy, cx, cy = intrinsics(w, h)
     if tex_scale is None:
         tex_scale = fx / plane_z          # texture pixels per world unit: ~1 texel per image pixel
     R, t = pose
     u, v = np.meshgrid(np.arange(w, dtype=np.float64), np.arange(h, dtype=np.float64))
-    rays = np.stack([(u - cx) / fx, (v - cy) / fy, np.ones_like(u)], -1) @ R.T
+    if dist is None:
+        rays = np.stack([(u - cx) / fx, (v - cy) / fy, np.ones_like(u)], -1) @ R.T
+    else:
+        x, y = undistort_normalised((u - cx) / fx, (v - cy) / fy, dist)
+        rays = np.stack([x, y, np.ones_like(u)], -1) @ R.T
     s = (plane_z - t[2]) / rays[..., 2]
     X = t[0] + s * rays[..., 0]
     Y = t[1] + s * rays[..., 1]
@@ -97,11 +119,12 @@ def gray_to_rgba(g):
     return out
 
 
-def make_frames(nframes, w, h, seed=99, rgba=True, texture_seed=1234):
-    """`seed` picks the camera path, `texture_seed` the scene (two calls with the same texture_seed look at the same plane)."""
+def make_frames(nframes, w, h, seed=99, rgba=True, texture_seed=1234, dist=None):
+    """`seed` picks the camera path, `texture_seed` the scene (two calls with the same texture_seed look at the same plane);
+    dist = (k1, k2, p1, p2) renders through OpenCV's radial-tangential lens with the intrinsics() camera (None: a pinhole)."""
     tex = make_texture(seed=texture_seed)
     poses = trajectory(nframes, w, h, seed)
-    frames = [render_gray(tex, p, w, h) for p in poses]
+    frames = [render_gray(tex, p, w, h, dist=dist) for p in poses]
     g = np.stack(frames)
     return (gray_to_rgba(g) if rgba else g), poses
 

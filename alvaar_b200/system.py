@@ -18,6 +18,7 @@ def _bind():
     L.alva_system_destroy.argtypes = [_vp]
     L.alva_system_reset.argtypes = [_vp]
     L.alva_system_set_clahe.argtypes = [_vp, _i32, _f64, _i32]
+    L.alva_system_set_distortion.argtypes = [_vp] + [_f64] * 4
     L.alva_system_num_matched.argtypes = [_vp]
     L.alva_system_configure.argtypes = [_vp, _i32, _i32] + [_f64] * 8
     L.alva_system_find_camera_pose.argtypes = [_vp, _vp, _vp]
@@ -129,3 +130,11 @@ class System:
         rc = self.L.alva_system_set_clahe(self.h, 1 if enabled else 0, float(clip_limit), int(tile_size))
         if rc != 0:
             raise AlvaError(f"alva_system_set_clahe -> {rc}: {self.L.alva_last_error().decode()}")
+
+    def set_distortion(self, k1, k2, p1, p2):
+        """OpenCV's radial-tangential lens model (the reference's configure(..., k1, k2, p1, p2)): keypoints are undistorted,
+        projections distorted, as the reference's CameraCalibration does.  Resets the tracker and the map; the next frame starts
+        under the new model.  Survives reset(); all zero is the pinhole camera."""
+        rc = self.L.alva_system_set_distortion(self.h, float(k1), float(k2), float(p1), float(p2))
+        if rc != 0:
+            raise AlvaError(f"alva_system_set_distortion -> {rc}: {self.L.alva_last_error().decode()}")

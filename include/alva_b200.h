@@ -83,6 +83,20 @@ int alva_k_scharr(alva_ctx*, const uint8_t* gray, int16_t* deriv, int w, int h, 
  * tiles < 1, tiles > the image size on either axis, or a negative / NaN clip_limit. */
 int alva_k_clahe(alva_ctx*, const uint8_t* src, uint8_t* dst, int w, int h, int nframes, double clip_limit, int tiles_x, int tiles_y);
 
+/* Lens distortion: OpenCV's radial-tangential model with D4 = {k1, k2, p1, p2}, as the reference's CameraCalibration applies it
+ * (camera_calibration.cpp:34-72), bit-exact.  K4 = {fx, fy, cx, cy} and D4 are HOST arrays (read at the call); the points are
+ * DEVICE buffers.  ALVA_E_INVALID for null pointers, non-finite K4 / D4, fx or fy == 0, or misaligned point buffers.
+ *
+ * alva_k_undistort_points: cv::undistortPoints(px, unpx, K, D, K) -- 5 fixed-point iterations, the pinhole fallback where the
+ * model folds back, the result in pixels -- for every keypoint px [nframes][cap][2] float (8-byte aligned); counts [nframes]
+ * (DEVICE, optional: NULL = cap points per frame) limits each frame.  unpx [nframes][cap][2] float; entries past a frame's count
+ * are not written.
+ * alva_k_project_points: CameraCalibration::projectCamToImageDist for n camera-frame points Xc [n][3] double: the normalised
+ * point is rounded to a cv::Point3f and projected with cv::projectPoints; uv [n][2] float (8-byte aligned). */
+int alva_k_undistort_points(alva_ctx*, const float* px, const int32_t* counts, int nframes, int cap, const double* K4,
+                            const double* D4, float* unpx);
+int alva_k_project_points(alva_ctx*, const double* Xc, int n, const double* K4, const double* D4, float* uv);
+
 /* cv::FAST(gray, thr, nms=true, TYPE_9_16) on each frame (opencv features2d/src/fast.cpp:496).
  * keys[f*cap + i]: packed corner keys; counts[f] = true number found (may exceed cap: then only cap
  * are stored and the call returns ALVA_E_CAPACITY after completing).  sorted != 0: row-major order. */
@@ -245,7 +259,7 @@ int alva_k_triangulate(alva_ctx*, const double* Tlr, const double* bvl, const do
  *   map point table: mp_wpt [n_mp][3], mp_is3d [n_mp], observations CSR obs_start [n_mp + 1] -> obs_kf (keyframe INDEX,
  *   ascending keyframe id) / obs_px [..][2], descriptors CSR desc_start [n_mp + 1] -> desc [..][32] (16-byte aligned);
  *   local_mp [n_local] = table indices of the local map in the host's iteration order (that order decides ties, as the
- *   reference's unordered_set order does).  Zero lens distortion (what the JS shim passes).
+ *   reference's unordered_set order does).  Zero lens distortion (what the JS shim passes; see alva_k_match_to_map_dist).
  * Out: kp_match [n_kp] = table index of the matched local map point or -1, kp_dist (optional) its Hamming distance,
  * n_match [1] the number of matched keypoints. */
 int alva_k_match_to_map(alva_ctx*, int w, int h, int cell, double fx, double fy, double cx, double cy, const double* Twc_cur,
@@ -253,6 +267,15 @@ int alva_k_match_to_map(alva_ctx*, int w, int h, int cell, double fx, double fy,
                         const double* mp_wpt, const uint8_t* mp_is3d, const int32_t* obs_start, const int32_t* obs_kf,
                         const float* obs_px, const int32_t* desc_start, const uint8_t* desc, int n_local, const int32_t* local_mp,
                         float max_proj_err, float dist_ratio, int32_t* kp_match, float* kp_dist, int32_t* n_match);
+/* The same with lens distortion: dist4 = {k1, k2, p1, p2} (HOST array; NULL or all zero = alva_k_match_to_map) is applied to
+ * the map point's projection and to the co-projection errors, as the reference's Frame::projCamToImageDist /
+ * projWorldToImageDist do (mapper.cpp:425, 504).  ALVA_E_INVALID for a non-finite coefficient. */
+int alva_k_match_to_map_dist(alva_ctx*, int w, int h, int cell, double fx, double fy, double cx, double cy, const double* Twc_cur,
+                             int n_kp, const int32_t* kp_mp, const float* kp_px, int nkp3d, int n_kf, const double* kf_Twc, int n_mp,
+                             const double* mp_wpt, const uint8_t* mp_is3d, const int32_t* obs_start, const int32_t* obs_kf,
+                             const float* obs_px, const int32_t* desc_start, const uint8_t* desc, int n_local, const int32_t* local_mp,
+                             float max_proj_err, float dist_ratio, int32_t* kp_match, float* kp_dist, int32_t* n_match,
+                             const double* dist4);
 
 /* Local bundle adjustment, batched over nprob independent problems of identical dimensions
  * (Optimizer::localBA, src/slam/src/optimizer.cpp:4-531, solved the way ceres::Solve does with the reference's
@@ -390,6 +413,12 @@ int  alva_system_reset(alva_system*);
  * it; it applies from the next frame.  ALVA_E_STATE before configure; ALVA_E_INVALID for an empty grid (tile_size > w or h, or
  * < 1) or, when enabling, a negative / NaN clip_limit. */
 int  alva_system_set_clahe(alva_system*, int enabled, double clip_limit, int tile_size);
+/* Lens distortion of a configured System: the reference's configure(..., k1, k2, p1, p2) coefficients (OpenCV's radial-tangential
+ * model), applied where its CameraCalibration applies them -- every tracked and detected keypoint is undistorted (on the device),
+ * the KLT priors of 3-D keypoints and the local-map matcher's projections are distorted.  It resets the tracker and the map as
+ * reset() does; the next frame starts under the new model.  All zero = the pinhole camera.  configure clears it, reset keeps it.
+ * ALVA_E_STATE before configure; ALVA_E_INVALID for a null handle or a non-finite coefficient. */
+int  alva_system_set_distortion(alva_system*, double k1, double k2, double p1, double p2);
 int  alva_system_find_camera_pose(alva_system*, const uint8_t* rgba, float* pose16);
 /* the same with the frame's time stamp (milliseconds) supplied by the caller instead of read from the system clock
  * (system.cpp:114): deterministic replays, and hosts that deliver frames faster than real time (two frames inside one
