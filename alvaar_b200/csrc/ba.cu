@@ -11,8 +11,8 @@
 //   LM shell          LevenbergMarquardtStrategy, TrustRegionMinimizer         levenberg_marquardt_strategy.cc:66-160, trust_region_minimizer.cc
 //
 // FP64 throughout (the north-star tolerance is 1e-4 relative; we land at ~1e-9).  The e-blocks are 1-dimensional
-// (inverse depth), so (E'E)^-1 is a scalar reciprocal per landmark; the reduced system is <= 20 poses x 6 = 120 wide
-// and lives in ONE CTA's shared memory for the (blocked) Cholesky / triangular solves; the Schur complement itself is
+// (inverse depth), so (E'E)^-1 is a scalar reciprocal per landmark; the reduced system is <= 21 free poses x 6 = 126 wide
+// (a problem with more is refused, termination 2) and lives in ONE CTA's shared memory for the (blocked) Cholesky / triangular solves; the Schur complement itself is
 // assembled block-wise by a gather kernel (one warp per 6x6 pose-pair block, no atomics, bit-reproducible).  The trust-region decisions
 // (accept / reject, radius update, function / parameter / gradient tolerance) run in single-CTA "control" kernels
 // that read and write a device-resident state block, so an entire solve is a fixed launch sequence with no host
@@ -277,8 +277,10 @@ __global__ void __launch_bounds__(SETUP_THREADS) ba_setup_kernel(const BaProblem
         if (c > 6 * NBMAX) {
             // more free poses than the reduced-system buffers hold (NBMAX): refuse the problem -- every later kernel returns at
             // once for a finished problem and the parameters stay untouched -- instead of writing past S / rhs.  term 2 = failure.
+            // ba_pre_body never runs, so the costs are set here: the summary reads 0, 0 rather than what the workspace last held.
             for (int k = 0; k < D.nkf; k++) P.pose_col[k] = -1;
             s.ncols = 0; s.nb = 0; s.done = 1; s.term = 2;
+            s.initial_cost = 0; s.x_cost = 0;
         }
     }
     // exclusive scan of counts -> lm_start
@@ -1217,7 +1219,8 @@ __global__ void __launch_bounds__(BS_THREADS) ba_backsub_kernel(const BaProblem*
     __shared__ double red[BS_THREADS];
     if (P.st->done) return;
     const int l = blockIdx.x * BS_THREADS + threadIdx.x;
-    if (blockIdx.x == 0 && (int)threadIdx.x < D.nkf) backsub_cand_pose(P, threadIdx.x, P.cand_poses + 7 * threadIdx.x);
+    if (blockIdx.x == 0)   // every keyframe (up to 256, two per thread): ba_post_body copies all nkf candidates over the poses
+        for (int k = threadIdx.x; k < D.nkf; k += BS_THREADS) backsub_cand_pose(P, k, P.cand_poses + 7 * k);
     const double acc = l < D.nlm ? backsub_landmark(P, l) : 0.0;
     const double tot = block_sum<BS_THREADS>(acc, red);
     if (threadIdx.x == 0) P.mc_part[blockIdx.x] = tot;

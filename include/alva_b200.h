@@ -304,8 +304,13 @@ int alva_k_ba_solve(alva_ctx*, int nprob, int nkf, int nlm, int nobs, const doub
  * obs_lm is not modified; flags [nprob][nobs] int32 (0 = inlier / unused slot); summary (optional) [nprob][10]:
  * {initial cost, final cost, #successful, #iterations, termination} of solve 1, then of solve 2 (zeros if skipped).
  * The reference's 1 ms wall-clock cap on step 3 (and 5 ms on step 1) is lifted, as everywhere in this library.
- * Size limit (alva_k_ba_solve too): at most 21 free (non-constant, referenced) poses per problem -- the reduced camera system
- * is factored in one CTA's shared memory; a problem with more is refused (termination 2, parameters untouched). */
+ * Size limits (alva_k_ba_solve too): 1 <= nkf <= 256 (else ALVA_E_INVALID), and at most 21 free (non-constant, referenced)
+ * poses per problem -- the reduced camera system is factored in one CTA's shared memory.  A problem with more free poses is
+ * refused, alone (the rest of the batch is solved): its parameters are untouched and its summary reads initial and final
+ * cost 0, 0 successful steps, 0 iterations, termination 2 (alva_k_ba_solve: width 0, radius 1e4, last iteration 0).
+ * alva_k_ba_local still tests the outliers, at the untouched input, and removes them (flags 1); if it removed any and
+ * huber_delta > 0, the second solve runs on the residuals left, and is refused the same way (summary[5..9] = 0, 0, 0, 0, 2)
+ * while they still reference more than 21 free poses. */
 int alva_k_ba_local(alva_ctx*, int nprob, int nkf, int nlm, int nobs, const double* calib, double* poses,
                     const uint8_t* pose_const, double* invd, const int32_t* anch_kf, const double* anch_uv,
                     const int32_t* obs_kf, const int32_t* obs_lm, const double* obs_uv, double huber_delta, double chi2_thr,
