@@ -54,7 +54,7 @@ struct BaProblem {
     const int32_t* obs_lm;     // [nobs]  (-1 = unused slot)
     const double* obs_uv;      // [nobs*2]
     // workspace
-    double *res, *Ja, *Jp, *Jd;             // per obs: 2, 12, 12, 2
+    double *res, *Ja, *Jd;                  // per obs: 2, 12, 2 (the observer's Jacobian is -Ja exactly: see ba_evaluate)
     double *wp;                             // per obs: 6  (F_p^T e)
     double *nf, *gf, *scf, *diagf, *Df;     // [NMAX]
     double *ne, *ge, *sce, *diage, *De;     // [nlm]
@@ -143,7 +143,9 @@ __device__ void se3_plus(const double* x, const double* delta, double* out) {
     for (int i = 0; i < 4; i++) out[3 + i] = q[i] / n;
 }
 
-// ReprojectionErrorKSE3AnchInvDepth::Evaluate; Ja/Jp are the LOCAL 2x6 Jacobians (J_global * [I6; 0])
+// ReprojectionErrorKSE3AnchInvDepth::Evaluate; Ja/Jp are the LOCAL 2x6 Jacobians (J_global * [I6; 0]).  Jp is Ja negated, entry
+// for entry and bit for bit (negation is exact, also after the Huber scaling), so the solver's workspace keeps Ja alone and reads
+// -Ja for the observer: 16 instead of 28 doubles per observation to write and read back every iteration.
 __device__ __forceinline__ bool ba_evaluate(const double* calib, const double* anch, const double* pose, double invd, double u,
                                             double v, double ua, double va, double* res, double* Ja, double* Jp, double* Jd) {
     const double fx = calib[0], fy = calib[1], cx = calib[2], cy = calib[3];
@@ -398,7 +400,7 @@ __device__ __forceinline__ double lin_obs(const BaProblem& P, const BaDims& D, i
         Jd[0] *= sc; Jd[1] *= sc;
         P.Jd[2 * o] = Jd[0]; P.Jd[2 * o + 1] = Jd[1];
 #pragma unroll
-        for (int i = 0; i < 12; i++) { Ja[i] *= sc; Jp[i] *= sc; P.Ja[12 * o + i] = Ja[i]; P.Jp[12 * o + i] = Jp[i]; }
+        for (int i = 0; i < 12; i++) { Ja[i] *= sc; P.Ja[12 * o + i] = Ja[i]; }   // Jp = -Ja: not stored
     }
     return 0.5 * rho0;
 }
@@ -447,7 +449,7 @@ __device__ __forceinline__ void stats_pose_partial(const BaProblem& P, int b, in
             const double r0 = P.res[2 * o], r1 = P.res[2 * o + 1];
 #pragma unroll
             for (int c = 0; c < 6; c++) {
-                const double j0 = P.Jp[12 * o + c], j1 = P.Jp[12 * o + 6 + c];
+                const double j0 = -P.Ja[12 * o + c], j1 = -P.Ja[12 * o + 6 + c];
                 v[c] += j0 * j0 + j1 * j1;
                 v[6 + c] += j0 * r0 + j1 * r1;
             }
@@ -712,7 +714,7 @@ __device__ void schur_landmark(const BaProblem& P, const BaDims& D, int l) {
         for (int c = 0; c < 6; c++) {
             Fa[c] = P.Ja[12 * o + c] * sca[c]; Fa[6 + c] = P.Ja[12 * o + 6 + c] * sca[c];
             const double s = cp >= 0 ? P.scf[cp + c] : 0.0;
-            Fp[c] = P.Jp[12 * o + c] * s; Fp[6 + c] = P.Jp[12 * o + 6 + c] * s;
+            Fp[c] = -P.Ja[12 * o + c] * s; Fp[6 + c] = -P.Ja[12 * o + 6 + c] * s;
         }
         for (int c = 0; c < 6; c++) {
             wa[c] += e0 * Fa[c] + e1 * Fa[6 + c];
@@ -875,7 +877,7 @@ __device__ __forceinline__ void lm_landmark(const BaProblem& P, int l) {
         etb += e0 * P.res[2 * o] + e1 * P.res[2 * o + 1];
         for (int c = 0; c < 6; c++) {
             if (ca >= 0) wa[c] += (e0 * P.Ja[12 * o + c] + e1 * P.Ja[12 * o + 6 + c]) * P.scf[ca + c];
-            P.wp[6 * o + c] = cp >= 0 ? (e0 * P.Jp[12 * o + c] + e1 * P.Jp[12 * o + 6 + c]) * P.scf[cp + c] : 0.0;
+            P.wp[6 * o + c] = cp >= 0 ? (e0 * -P.Ja[12 * o + c] + e1 * -P.Ja[12 * o + 6 + c]) * P.scf[cp + c] : 0.0;
         }
     }
     P.ete[l] = ete;
@@ -935,7 +937,7 @@ __device__ __forceinline__ void gather_entry(const BaProblem& P, uint64_t en, co
     } else if (su == sv) {                           // observation x itself
         double F0[6], F1[6];
 #pragma unroll
-        for (int c = 0; c < 6; c++) { F0[c] = P.Jp[12 * ou + c] * sci[c]; F1[c] = P.Jp[12 * ou + 6 + c] * sci[c]; }
+        for (int c = 0; c < 6; c++) { F0[c] = -P.Ja[12 * ou + c] * sci[c]; F1[c] = -P.Ja[12 * ou + 6 + c] * sci[c]; }
         const double r0 = P.res[2 * ou], r1 = P.res[2 * ou + 1];
 #pragma unroll
         for (int a = 0; a < 6; a++) {
@@ -948,13 +950,13 @@ __device__ __forceinline__ void gather_entry(const BaProblem& P, uint64_t en, co
         double A0[6], A1[6];
 #pragma unroll
         for (int a = 0; a < 6; a++) {
-            A0[a] = (su ? P.Jp[12 * o + a] : P.Ja[12 * o + a]) * sci[a];
-            A1[a] = (su ? P.Jp[12 * o + 6 + a] : P.Ja[12 * o + 6 + a]) * sci[a];
+            A0[a] = (su ? -P.Ja[12 * o + a] : P.Ja[12 * o + a]) * sci[a];
+            A1[a] = (su ? -P.Ja[12 * o + 6 + a] : P.Ja[12 * o + 6 + a]) * sci[a];
         }
 #pragma unroll
         for (int c = 0; c < 6; c++) {
-            const double b0 = (sv ? P.Jp[12 * o + c] : P.Ja[12 * o + c]) * scj[c];
-            const double b1 = (sv ? P.Jp[12 * o + 6 + c] : P.Ja[12 * o + 6 + c]) * scj[c];
+            const double b0 = (sv ? -P.Ja[12 * o + c] : P.Ja[12 * o + c]) * scj[c];
+            const double b1 = (sv ? -P.Ja[12 * o + 6 + c] : P.Ja[12 * o + 6 + c]) * scj[c];
 #pragma unroll
             for (int a = 0; a < 6; a++) ACC(a, c) += A0[a] * b0 + A1[a] * b1;
         }
@@ -1051,10 +1053,12 @@ __global__ void __launch_bounds__(GA_THREADS, 8) ba_gather_kernel(const BaProble
 // ------------------------------------------------------------------------------------------ reduced solve (1 CTA / problem)
 // Right-looking LDL' of the <= 126 x 126 reduced camera system, REGISTER-TILED: the lower triangle of the (augmented) 128 x 128
 // matrix is cut into 4 x 4 tiles, one per thread (528 tiles, column-block-major, so whole warps retire as the elimination moves
-// right); V = L D is built in place.  Per column j: the threads holding it publish the column through shared memory (double
-// buffered: ONE barrier per column), then every live tile takes its rank-1 update  a[i][c] -= V[i][j] (V[c][j] / d_j)  from 8
-// shared-memory words -- 16 FP64 FMAs against 8 loads, where a left-looking form spends three loads per multiply-add and is
-// shared-memory-bandwidth bound.  Row n of the matrix is the right-hand side, so the
+// right); V = L D is built in place.  Per panel of 4 columns (one tile column), TWO barriers: the diagonal tile eliminates its
+// 4 x 4 block in registers and publishes it with the 4 pivot reciprocals; the tiles below it finish their 4 columns locally and
+// publish them; then every trailing tile takes the 4 rank-1 updates  a[i][c] -= V[i][j] (V[c][j] / d_j)  in column order, from
+// 8 shared-memory words each -- 16 FP64 FMAs against 8 loads, where a left-looking form spends three loads per multiply-add and
+// is shared-memory-bandwidth bound.  Each element gets the same products subtracted in the same order as with one barrier
+// per column, so the result is the same bits.  Row n of the matrix is the right-hand side, so the
 // forward substitution z = L^-1 b falls out of the same updates.  Then x = L^-T D^-1 z by warp 0 (lane-strided, registers).
 // No square roots; fixed operation order (bit-reproducible).  yf = S^-1 rhs.
 constexpr int CH_TILES = 32 * 33 / 2, CH_THREADS = (CH_TILES + 31) / 32 * 32;   // 528 tiles -> 544 threads
@@ -1065,8 +1069,9 @@ __device__ void ba_chol_body(const BaProblem& P, double* sm) {
     const int ld = NMAX + 1;
     double* V = sm;                 // (n + 1) x ld, filled after the factorisation for the backward solve
     double* invd = sm + NMAX * ld;  // NMAX
-    __shared__ double colbuf[2][NMAX];
-    __shared__ double pivinv[2];
+    __shared__ double pcol[4][NMAX];   // the panel's columns, rows below its diagonal tile
+    __shared__ double dg[4][4];        // the panel's diagonal tile, eliminated
+    __shared__ double pivinv[2][4];    // the panel's pivot reciprocals, by panel parity
     __shared__ int ok_s;
     // tile of this thread: column block tj, row block ti >= tj
     int tj = 0, rem = tid;
@@ -1089,45 +1094,76 @@ __device__ void ba_chol_body(const BaProblem& P, double* sm) {
         }
     if (tid == 0) ok_s = 1;
     const int last_jb = (n - 1) >> 2;
-    // a tile is live while columns of its own column block are still to be eliminated
+    // One panel (tile column jb, its 4 columns j = 4 jb + jj) per pass, two barriers.  Column-block-major tile order: a warp's
+    // lanes retire (tj < jb) almost together, and a retired warp only keeps arriving at the barriers.
     for (int jb = 0; jb <= last_jb; jb++) {
-        const bool live = tile && tj >= jb;   // column-block-major tile order: a warp's lanes drop out almost together, and a
-                                              // retired warp only keeps arriving at the barriers
+        const int nj = min(4, n - 4 * jb);   // columns of this panel (uniform)
+        double* pinv = pivinv[jb & 1];       // the next panel's diagonal tile writes the other half while trailing tiles read this one
+        // 1. the diagonal tile eliminates its 4 x 4 block in registers and publishes it with the pivot reciprocals
+        if (tile && ti == jb && tj == jb) {
 #pragma unroll
-        for (int jj = 0; jj < 4; jj++) {
-            const int j = 4 * jb + jj;
-            if (j >= n) break;   // uniform
-            double* cb = colbuf[j & 1];
-            if (live && tj == jb) {   // publish column j (rows >= j of it are final)
+            for (int jj = 0; jj < 4; jj++) {
+                if (jj >= nj) break;
+                const double d = a[jj][jj];
+                if (!(d > 0)) ok_s = 0;
+                // 1 / d sits on the serial chain of the elimination (pivot j + 1 needs it): MUFU.RCP64H seed (>= 20 bits) + two
+                // Newton steps = 5 dependent operations instead of the IEEE division's subroutine; error <= 1 ulp, fixed sequence
+                const double dd = d > 0 ? d : 1.0;
+                double inv;
+                asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(inv) : "d"(dd));
+                inv = fma(inv, fma(-dd, inv, 1.0), inv);
+                inv = fma(inv, fma(-dd, inv, 1.0), inv);
+                pinv[jj] = inv;
+                invd[4 * jb + jj] = inv;
+                double lc[4];
 #pragma unroll
-                for (int r = 0; r < 4; r++) cb[r0 + r] = a[r][jj];
-                if (ti == tj) {
-                    const double d = a[jj][jj];
-                    if (!(d > 0)) ok_s = 0;
-                    // 1 / d sits on the serial chain of the elimination (pivot j + 1 needs it): MUFU.RCP64H seed (>= 20 bits) + two
-                    // Newton steps = 5 dependent operations instead of the IEEE division's subroutine; error <= 1 ulp, fixed sequence
-                    const double dd = d > 0 ? d : 1.0;
-                    double inv;
-                    asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(inv) : "d"(dd));
-                    inv = fma(inv, fma(-dd, inv, 1.0), inv);
-                    inv = fma(inv, fma(-dd, inv, 1.0), inv);
-                    pivinv[j & 1] = inv;
-                    invd[j] = inv;
-                }
-            }
-            __syncthreads();
-            if (live) {
-                const double inv = pivinv[j & 1];
-                double lr[4], lc[4];
-#pragma unroll
-                for (int r = 0; r < 4; r++) lr[r] = cb[r0 + r];
-#pragma unroll
-                for (int c = 0; c < 4; c++) lc[c] = cb[c0 + c] * inv;
+                for (int c = 0; c < 4; c++) lc[c] = a[c][jj] * inv;
 #pragma unroll
                 for (int r = 0; r < 4; r++)
 #pragma unroll
-                    for (int c = 0; c < 4; c++)
-                        if (tj > jb || c > jj) a[r][c] -= lr[r] * lc[c];   // columns right of j only (tj == jb: compile-time c > jj)
+                    for (int c = jj + 1; c < 4; c++) a[r][c] -= a[r][jj] * lc[c];
+            }
+#pragma unroll
+            for (int r = 0; r < 4; r++)
+#pragma unroll
+                for (int c = 0; c < 4; c++) dg[r][c] = a[r][c];
+        }
+        __syncthreads();
+        // 2. the panel's tiles below it apply the in-panel updates and publish their 4 finished columns
+        if (tile && tj == jb && ti > jb) {
+#pragma unroll
+            for (int jj = 0; jj < 4; jj++) {
+                if (jj >= nj) break;
+                double lc[4];
+#pragma unroll
+                for (int c = 0; c < 4; c++) lc[c] = dg[c][jj] * pinv[jj];
+#pragma unroll
+                for (int r = 0; r < 4; r++)
+#pragma unroll
+                    for (int c = jj + 1; c < 4; c++) a[r][c] -= a[r][jj] * lc[c];
+            }
+#pragma unroll
+            for (int jj = 0; jj < 4; jj++)
+#pragma unroll
+                for (int r = 0; r < 4; r++) pcol[jj][r0 + r] = a[r][jj];
+        }
+        __syncthreads();
+        // 3. the trailing tiles take the panel's rank-1 updates  a[i][c] -= V[i][j] (V[c][j] / d_j)  in column order -- every
+        // element sees the same products subtracted in the same order as a column-at-a-time elimination
+        if (tile && tj > jb) {
+#pragma unroll
+            for (int jj = 0; jj < 4; jj++) {
+                if (jj >= nj) break;
+                const double inv = pinv[jj];
+                double lr[4], lc[4];
+#pragma unroll
+                for (int r = 0; r < 4; r++) lr[r] = pcol[jj][r0 + r];
+#pragma unroll
+                for (int c = 0; c < 4; c++) lc[c] = pcol[jj][c0 + c] * inv;
+#pragma unroll
+                for (int r = 0; r < 4; r++)
+#pragma unroll
+                    for (int c = 0; c < 4; c++) a[r][c] -= lr[r] * lc[c];
             }
         }
     }
@@ -1204,7 +1240,7 @@ __device__ __forceinline__ double backsub_landmark(const BaProblem& P, int l) {
             double m0 = P.Jd[2 * o] * se, m1 = P.Jd[2 * o + 1] * se;
             for (int c = 0; c < 6; c++) {
                 if (ca >= 0) { const double q = -P.yf[ca + c] * P.scf[ca + c]; m0 += P.Ja[12 * o + c] * q; m1 += P.Ja[12 * o + 6 + c] * q; }
-                if (cp >= 0) { const double q = -P.yf[cp + c] * P.scf[cp + c]; m0 += P.Jp[12 * o + c] * q; m1 += P.Jp[12 * o + 6 + c] * q; }
+                if (cp >= 0) { const double q = -P.yf[cp + c] * P.scf[cp + c]; m0 += -P.Ja[12 * o + c] * q; m1 += -P.Ja[12 * o + 6 + c] * q; }
             }
             acc += m0 * (P.res[2 * o] + m0 / 2.0) + m1 * (P.res[2 * o + 1] + m1 / 2.0);
         }
@@ -1400,7 +1436,7 @@ static int g_ba_ctl_threads = CT_THREADS;   // alva_set_option("ba_ctl_threads",
 static size_t ba_ws_bytes(int nkf, int nlm, int nobs, int nblk) {
     size_t d = 0;
     if (g_ba_dense_schur) d += (size_t)((nlm + 3) / 4 * 4) * NMAX;
-    d += (size_t)nobs * (2 + 12 + 12 + 2 + 6);      // res, Ja, Jp, Jd, wp
+    d += (size_t)nobs * (2 + 12 + 2 + 6);           // res, Ja, Jd, wp
     d += 5 * (size_t)NMAX;                           // nf gf scf diagf Df
     d += 5 * (size_t)nlm;                            // ne ge sce diage De
     d += (size_t)nlm * (1 + 1 + 6 + 1);              // ete etb wa ye
@@ -1454,7 +1490,7 @@ static int ba_prepare(alva_ctx* ctx, int nprob, int nkf, int nlm, int nobs, cons
             P.obs_kf = obs_kf + (size_t)nobs * p; P.obs_lm = obs_lm + (size_t)nobs * p; P.obs_uv = obs_uv + 2 * (size_t)nobs * p;
             double* d = reinterpret_cast<double*>(ws + tab + per * p);
             auto take = [&](size_t n) { double* r = d; d += n; return r; };
-            P.res = take(2 * (size_t)nobs); P.Ja = take(12 * (size_t)nobs); P.Jp = take(12 * (size_t)nobs); P.Jd = take(2 * (size_t)nobs);
+            P.res = take(2 * (size_t)nobs); P.Ja = take(12 * (size_t)nobs); P.Jd = take(2 * (size_t)nobs);
             P.wp = take(6 * (size_t)nobs);
             P.nf = take(NMAX); P.gf = take(NMAX); P.scf = take(NMAX); P.diagf = take(NMAX); P.Df = take(NMAX);
             P.ne = take(nlm); P.ge = take(nlm); P.sce = take(nlm); P.diage = take(nlm); P.De = take(nlm);
