@@ -194,6 +194,21 @@ __device__ __forceinline__ void huber(double s, double delta, double& rho0, doub
     } else { rho0 = s; rho1 = 1.0; }
 }
 
+// 16-byte loads / stores of the workspace's per-observation records (res, Jd: 2 doubles; Ja: 12; wp: 6) and per-landmark F'e (wa: 6).
+// Every workspace array starts 16-byte aligned (ba_prepare) and every record is an even number of doubles, so a record moves in
+// N / 2 vector accesses instead of N scalar ones: half the memory instructions and L2 requests, the same values.  The BA kernels
+// that read these records per observation or per Schur entry issue little else.
+template <int N>
+__device__ __forceinline__ void ld2(const double* p, double* v) {
+#pragma unroll
+    for (int i = 0; i < N / 2; i++) { const double2 t = reinterpret_cast<const double2*>(p)[i]; v[2 * i] = t.x; v[2 * i + 1] = t.y; }
+}
+template <int N>
+__device__ __forceinline__ void st2(double* p, const double* v) {
+#pragma unroll
+    for (int i = 0; i < N / 2; i++) reinterpret_cast<double2*>(p)[i] = make_double2(v[2 * i], v[2 * i + 1]);
+}
+
 // deterministic block reduction (fixed tree), result valid in thread 0
 template <int NT>
 __device__ __forceinline__ double block_sum(double v, double* sm) {
@@ -396,11 +411,12 @@ __device__ __forceinline__ double lin_obs(const BaProblem& P, const BaDims& D, i
     if (FULL) {
         const double sc = sqrt(rho1);
         r[0] *= sc; r[1] *= sc;
-        P.res[2 * o] = r[0]; P.res[2 * o + 1] = r[1];
+        st2<2>(P.res + 2 * o, r);
         Jd[0] *= sc; Jd[1] *= sc;
-        P.Jd[2 * o] = Jd[0]; P.Jd[2 * o + 1] = Jd[1];
+        st2<2>(P.Jd + 2 * o, Jd);
 #pragma unroll
-        for (int i = 0; i < 12; i++) { Ja[i] *= sc; P.Ja[12 * o + i] = Ja[i]; }   // Jp = -Ja: not stored
+        for (int i = 0; i < 12; i++) Ja[i] *= sc;
+        st2<12>(P.Ja + 12 * o, Ja);   // Jp = -Ja: not stored
     }
     return 0.5 * rho0;
 }
@@ -425,9 +441,11 @@ __device__ __forceinline__ void stats_landmark(const BaProblem& P, int l) {
     double ne = 0, ge = 0;
     for (int i = P.lm_start[l]; i < P.lm_start[l + 1]; i++) {
         const int o = P.lm_obs[i];
-        const double d0 = P.Jd[2 * o], d1 = P.Jd[2 * o + 1];
-        ne += d0 * d0 + d1 * d1;
-        ge += d0 * P.res[2 * o] + d1 * P.res[2 * o + 1];
+        double d[2], q[2];
+        ld2<2>(P.Jd + 2 * o, d);
+        ld2<2>(P.res + 2 * o, q);
+        ne += d[0] * d[0] + d[1] * d[1];
+        ge += d[0] * q[0] + d[1] * q[1];
     }
     P.ne[l] = ne;
     P.ge[l] = ge;
@@ -446,20 +464,26 @@ __device__ __forceinline__ void stats_pose_partial(const BaProblem& P, int b, in
         const int ob = P.lm_start[l];
         if (su) {
             const int o = P.lm_obs[ob + su - 1];
-            const double r0 = P.res[2 * o], r1 = P.res[2 * o + 1];
+            double q[2], J[12];
+            ld2<2>(P.res + 2 * o, q);
+            ld2<12>(P.Ja + 12 * o, J);
+            const double r0 = q[0], r1 = q[1];
 #pragma unroll
             for (int c = 0; c < 6; c++) {
-                const double j0 = -P.Ja[12 * o + c], j1 = -P.Ja[12 * o + 6 + c];
+                const double j0 = -J[c], j1 = -J[6 + c];
                 v[c] += j0 * j0 + j1 * j1;
                 v[6 + c] += j0 * r0 + j1 * r1;
             }
         } else {
             for (int i = ob; i < P.lm_start[l + 1]; i++) {
                 const int o = P.lm_obs[i];
-                const double r0 = P.res[2 * o], r1 = P.res[2 * o + 1];
+                double q[2], J[12];
+                ld2<2>(P.res + 2 * o, q);
+                ld2<12>(P.Ja + 12 * o, J);
+                const double r0 = q[0], r1 = q[1];
 #pragma unroll
                 for (int c = 0; c < 6; c++) {
-                    const double j0 = P.Ja[12 * o + c], j1 = P.Ja[12 * o + 6 + c];
+                    const double j0 = J[c], j1 = J[6 + c];
                     v[c] += j0 * j0 + j1 * j1;
                     v[6 + c] += j0 * r0 + j1 * r1;
                 }
@@ -872,17 +896,23 @@ __device__ __forceinline__ void lm_landmark(const BaProblem& P, int l) {
     for (int i = b; i < e; i++) {
         const int o = P.lm_obs[i];
         const int cp = P.pose_col[P.obs_kf[o]];
-        const double e0 = P.Jd[2 * o] * sce, e1 = P.Jd[2 * o + 1] * sce;
+        double d[2], q[2], J[12], w[6];
+        ld2<2>(P.Jd + 2 * o, d);
+        ld2<2>(P.res + 2 * o, q);
+        ld2<12>(P.Ja + 12 * o, J);
+        const double e0 = d[0] * sce, e1 = d[1] * sce;
         ete += e0 * e0 + e1 * e1;
-        etb += e0 * P.res[2 * o] + e1 * P.res[2 * o + 1];
+        etb += e0 * q[0] + e1 * q[1];
+#pragma unroll
         for (int c = 0; c < 6; c++) {
-            if (ca >= 0) wa[c] += (e0 * P.Ja[12 * o + c] + e1 * P.Ja[12 * o + 6 + c]) * P.scf[ca + c];
-            P.wp[6 * o + c] = cp >= 0 ? (e0 * -P.Ja[12 * o + c] + e1 * -P.Ja[12 * o + 6 + c]) * P.scf[cp + c] : 0.0;
+            if (ca >= 0) wa[c] += (e0 * J[c] + e1 * J[6 + c]) * P.scf[ca + c];
+            w[c] = cp >= 0 ? (e0 * -J[c] + e1 * -J[6 + c]) * P.scf[cp + c] : 0.0;
         }
+        st2<6>(P.wp + 6 * o, w);
     }
     P.ete[l] = ete;
     P.etb[l] = etb;
-    for (int c = 0; c < 6; c++) P.wa[6 * l + c] = wa[c];
+    st2<6>(P.wa + 6 * l, wa);
 }
 // ... or, for a problem whose structure the packed lists cannot express (use_gather == 0), the whole per-landmark Schur update with
 // FP64 atomics (one launch serves both paths: a problem takes exactly one of them)
@@ -905,11 +935,10 @@ __device__ __forceinline__ void gather_entry(const BaProblem& P, uint64_t en, co
     const double inv = 1.0 / P.ete[l], etb = P.etb[l];
     const int ou = su ? (int)(en >> 16) & 0xffff : -1, ov = sv ? (int)en & 0xffff : -1;
     double wu[6], wv[6];
+    ld2<6>(su ? P.wp + 6 * ou : P.wa + 6 * l, wu);
+    ld2<6>(sv ? P.wp + 6 * ov : P.wa + 6 * l, wv);
 #pragma unroll
-    for (int c = 0; c < 6; c++) {
-        wu[c] = (su ? P.wp[6 * ou + c] : P.wa[6 * l + c]) * inv;
-        wv[c] = sv ? P.wp[6 * ov + c] : P.wa[6 * l + c];
-    }
+    for (int c = 0; c < 6; c++) wu[c] *= inv;
 #define ACC(a, c) acc[TRANSPOSE ? 6 * (c) + (a) : 6 * (a) + (c)]
 #pragma unroll
     for (int a = 0; a < 6; a++)
@@ -920,10 +949,12 @@ __device__ __forceinline__ void gather_entry(const BaProblem& P, uint64_t en, co
         const int ob = P.lm_start[l], oe = P.lm_start[l + 1];
         for (int i = ob; i < oe; i++) {
             const int o = P.lm_obs[i];
-            double F0[6], F1[6];
+            double F0[6], F1[6], J[12], q[2];
+            ld2<12>(P.Ja + 12 * o, J);
+            ld2<2>(P.res + 2 * o, q);
 #pragma unroll
-            for (int c = 0; c < 6; c++) { F0[c] = P.Ja[12 * o + c] * sci[c]; F1[c] = P.Ja[12 * o + 6 + c] * sci[c]; }
-            const double r0 = P.res[2 * o], r1 = P.res[2 * o + 1];
+            for (int c = 0; c < 6; c++) { F0[c] = J[c] * sci[c]; F1[c] = J[6 + c] * sci[c]; }
+            const double r0 = q[0], r1 = q[1];
 #pragma unroll
             for (int a = 0; a < 6; a++) {
                 if (!TRANSPOSE) rh[a] += F0[a] * r0 + F1[a] * r1;
@@ -935,10 +966,12 @@ __device__ __forceinline__ void gather_entry(const BaProblem& P, uint64_t en, co
 #pragma unroll
             for (int a = 0; a < 6; a++) rh[a] -= wu[a] * etb;
     } else if (su == sv) {                           // observation x itself
-        double F0[6], F1[6];
+        double F0[6], F1[6], J[12], q[2];
+        ld2<12>(P.Ja + 12 * ou, J);
+        ld2<2>(P.res + 2 * ou, q);
 #pragma unroll
-        for (int c = 0; c < 6; c++) { F0[c] = -P.Ja[12 * ou + c] * sci[c]; F1[c] = -P.Ja[12 * ou + 6 + c] * sci[c]; }
-        const double r0 = P.res[2 * ou], r1 = P.res[2 * ou + 1];
+        for (int c = 0; c < 6; c++) { F0[c] = -J[c] * sci[c]; F1[c] = -J[6 + c] * sci[c]; }
+        const double r0 = q[0], r1 = q[1];
 #pragma unroll
         for (int a = 0; a < 6; a++) {
             if (!TRANSPOSE) rh[a] += F0[a] * r0 + F1[a] * r1 - wu[a] * etb;
@@ -947,16 +980,17 @@ __device__ __forceinline__ void gather_entry(const BaProblem& P, uint64_t en, co
         }
     } else if (su == 0 || sv == 0) {                 // anchor x observation (either order): rows of that observation
         const int o = su ? ou : ov;
-        double A0[6], A1[6];
+        double A0[6], A1[6], J[12];
+        ld2<12>(P.Ja + 12 * o, J);
 #pragma unroll
         for (int a = 0; a < 6; a++) {
-            A0[a] = (su ? -P.Ja[12 * o + a] : P.Ja[12 * o + a]) * sci[a];
-            A1[a] = (su ? -P.Ja[12 * o + 6 + a] : P.Ja[12 * o + 6 + a]) * sci[a];
+            A0[a] = (su ? -J[a] : J[a]) * sci[a];
+            A1[a] = (su ? -J[6 + a] : J[6 + a]) * sci[a];
         }
 #pragma unroll
         for (int c = 0; c < 6; c++) {
-            const double b0 = (sv ? -P.Ja[12 * o + c] : P.Ja[12 * o + c]) * scj[c];
-            const double b1 = (sv ? -P.Ja[12 * o + 6 + c] : P.Ja[12 * o + 6 + c]) * scj[c];
+            const double b0 = (sv ? -J[c] : J[c]) * scj[c];
+            const double b1 = (sv ? -J[6 + c] : J[6 + c]) * scj[c];
 #pragma unroll
             for (int a = 0; a < 6; a++) ACC(a, c) += A0[a] * b0 + A1[a] * b1;
         }
@@ -1226,23 +1260,28 @@ __device__ __forceinline__ double backsub_landmark(const BaProblem& P, int l) {
     if (e > b) {
         double s = P.etb[l];
         const int ca = P.pose_col[P.anch_kf[l]];
-        if (ca >= 0) for (int c = 0; c < 6; c++) s -= P.wa[6 * l + c] * P.yf[ca + c];
+        if (ca >= 0) { double w[6]; ld2<6>(P.wa + 6 * l, w); for (int c = 0; c < 6; c++) s -= w[c] * P.yf[ca + c]; }
         for (int i = b; i < e; i++) {
             const int o = P.lm_obs[i];
             const int cp = P.pose_col[P.obs_kf[o]];
-            if (cp >= 0) for (int c = 0; c < 6; c++) s -= P.wp[6 * o + c] * P.yf[cp + c];
+            if (cp >= 0) { double w[6]; ld2<6>(P.wp + 6 * o, w); for (int c = 0; c < 6; c++) s -= w[c] * P.yf[cp + c]; }
         }
         ye = s / P.ete[l];
         const double se = -ye * P.sce[l];
         for (int i = b; i < e; i++) {
             const int o = P.lm_obs[i];
             const int cp = P.pose_col[P.obs_kf[o]];
-            double m0 = P.Jd[2 * o] * se, m1 = P.Jd[2 * o + 1] * se;
+            double d[2], r[2], J[12];
+            ld2<2>(P.Jd + 2 * o, d);
+            ld2<2>(P.res + 2 * o, r);
+            ld2<12>(P.Ja + 12 * o, J);
+            double m0 = d[0] * se, m1 = d[1] * se;
+#pragma unroll
             for (int c = 0; c < 6; c++) {
-                if (ca >= 0) { const double q = -P.yf[ca + c] * P.scf[ca + c]; m0 += P.Ja[12 * o + c] * q; m1 += P.Ja[12 * o + 6 + c] * q; }
-                if (cp >= 0) { const double q = -P.yf[cp + c] * P.scf[cp + c]; m0 += -P.Ja[12 * o + c] * q; m1 += -P.Ja[12 * o + 6 + c] * q; }
+                if (ca >= 0) { const double q = -P.yf[ca + c] * P.scf[ca + c]; m0 += J[c] * q; m1 += J[6 + c] * q; }
+                if (cp >= 0) { const double q = -P.yf[cp + c] * P.scf[cp + c]; m0 += -J[c] * q; m1 += -J[6 + c] * q; }
             }
-            acc += m0 * (P.res[2 * o] + m0 / 2.0) + m1 * (P.res[2 * o + 1] + m1 / 2.0);
+            acc += m0 * (r[0] + m0 / 2.0) + m1 * (r[1] + m1 / 2.0);
         }
         P.cand_invd[l] = P.invd[l] + se;
     } else
@@ -1445,6 +1484,7 @@ static size_t ba_ws_bytes(int nkf, int nlm, int nobs, int nblk) {
     d += (size_t)nblk;                               // cost partials
     d += (size_t)((nlm + BS_THREADS - 1) / BS_THREADS);   // model-cost partials
     d += (size_t)NBMAX * GA_SPLIT * 42;                   // gather partials
+    d += 64;                                              // ba_prepare rounds every array to an even number of doubles
     size_t bytes = d * sizeof(double);
     bytes += align_up((size_t)nkf * 4, 8) + align_up((size_t)(nlm + 1) * 4, 8) + align_up((size_t)nobs * 4, 8);
     bytes += align_up((size_t)nobs * 4, 8) + align_up((size_t)nlm * 4, 8);                          // obs_col, anch_col
@@ -1489,7 +1529,7 @@ static int ba_prepare(alva_ctx* ctx, int nprob, int nkf, int nlm, int nobs, cons
             P.invd = invd + (size_t)nlm * p; P.anch_kf = anch_kf + (size_t)nlm * p; P.anch_uv = anch_uv + 2 * (size_t)nlm * p;
             P.obs_kf = obs_kf + (size_t)nobs * p; P.obs_lm = obs_lm + (size_t)nobs * p; P.obs_uv = obs_uv + 2 * (size_t)nobs * p;
             double* d = reinterpret_cast<double*>(ws + tab + per * p);
-            auto take = [&](size_t n) { double* r = d; d += n; return r; };
+            auto take = [&](size_t n) { double* r = d; d += (n + 1) & ~(size_t)1; return r; };   // every array 16-byte aligned (ld2)
             P.res = take(2 * (size_t)nobs); P.Ja = take(12 * (size_t)nobs); P.Jd = take(2 * (size_t)nobs);
             P.wp = take(6 * (size_t)nobs);
             P.nf = take(NMAX); P.gf = take(NMAX); P.scf = take(NMAX); P.diagf = take(NMAX); P.Df = take(NMAX);
@@ -1663,6 +1703,49 @@ extern "C" int alva_k_ba_linearize(alva_ctx* ctx, int nkf, int nlm, int nobs, co
     (void)nkf; (void)nlm;
     ba_linearize_dump_kernel<<<(nobs + 127) / 128, 128, 0, ctx->stream>>>(calib, poses, invd, anch_kf, anch_uv, obs_kf, obs_lm,
                                                                          obs_uv, nobs, huber_delta, res, Ja, Jp, Jd, cost_per_obs);
+    ALVA_LAUNCH_CHECK(ctx);
+    return 0;
+}
+
+// Test hook: the reduced camera system S, rhs of a solve's first LM iteration (iteration 0's linearisation, Jacobi scaling
+// and diagonal), assembled by the path the solve would take -- or, with atomic != 0, by the atomic per-landmark path on the
+// same linearisation.  S_out [nprob][128][128], rhs_out [nprob][128], info [nprob][2] = {reduced-system width, gather path}.
+namespace {
+__global__ void ba_force_atomic_kernel(const BaProblem* __restrict__ probs) { probs[blockIdx.x].st->use_gather = 0; }
+__global__ void ba_dump_schur_kernel(const BaProblem* __restrict__ probs, double* S_out, double* rhs_out, double* info) {
+    const BaProblem P = probs[blockIdx.x];
+    for (int i = threadIdx.x; i < NMAX * NMAX; i += blockDim.x) S_out[(size_t)blockIdx.x * NMAX * NMAX + i] = P.S[i];
+    for (int i = threadIdx.x; i < NMAX; i += blockDim.x) rhs_out[(size_t)blockIdx.x * NMAX + i] = P.rhs[i];
+    if (threadIdx.x == 0) { info[2 * blockIdx.x] = P.st->ncols; info[2 * blockIdx.x + 1] = P.st->use_gather; }
+}
+}  // namespace
+extern "C" int alva_k_ba_schur_dump(alva_ctx* ctx, int nprob, int nkf, int nlm, int nobs, const double* calib, const double* poses,
+                                    const uint8_t* pose_const, const double* invd, const int32_t* anch_kf, const double* anch_uv,
+                                    const int32_t* obs_kf, const int32_t* obs_lm, const double* obs_uv, double huber_delta,
+                                    int atomic, double* S_out, double* rhs_out, double* info) { AlvaDeviceGuard guard__(ctx);
+    if (!ba_args_ok(ctx, nprob, nkf, nlm, nobs, calib, poses, pose_const, invd, anch_kf, anch_uv, obs_kf, obs_lm, obs_uv, 1) ||
+        !S_out || !rhs_out || !info || g_ba_dense_schur) {
+        alva_set_error("alva_k_ba_schur_dump: bad argument (need 1 <= nkf <= 256, outputs, ba_dense_schur off)");
+        return ALVA_E_INVALID;
+    }
+    const BaProblem* dp;
+    BaDims D;
+    // the first iteration writes neither the poses nor the inverse depths (only ba_post_kernel does)
+    if (int e = ba_prepare(ctx, nprob, nkf, nlm, nobs, calib, const_cast<double*>(poses), pose_const, const_cast<double*>(invd),
+                           anch_kf, anch_uv, obs_kf, obs_lm, obs_uv, nullptr, &dp, &D))
+        return e;
+    D.huber = huber_delta; D.max_iter = 1;
+    const dim3 lin_grid(D.nblk, nprob), schur_grid((D.nlm_pad + 127) / 128, nprob), stats_grid(D.nbs + NBMAX, nprob);
+    ba_setup_kernel<<<nprob, SETUP_THREADS, 0, ctx->stream>>>(dp, D);
+    ba_pairs_kernel<0><<<dim3(NBMAX, nprob), 32, 0, ctx->stream>>>(dp, D);
+    ba_pairs_kernel<1><<<dim3(NBMAX, nprob), 32, 0, ctx->stream>>>(dp, D);
+    if (atomic) ba_force_atomic_kernel<<<nprob, 1, 0, ctx->stream>>>(dp);
+    ba_linearize_kernel<true><<<lin_grid, LIN_THREADS, 0, ctx->stream>>>(dp, D);
+    ba_stats_kernel<<<stats_grid, BS_THREADS, 0, ctx->stream>>>(dp, D);
+    ba_pre_kernel<<<nprob, g_ba_ctl_threads, 0, ctx->stream>>>(dp, D);
+    ba_lm_kernel<<<schur_grid, 128, 0, ctx->stream>>>(dp, D);
+    ba_gather_kernel<<<dim3(GA_GRID, nprob), GA_THREADS, 0, ctx->stream>>>(dp, D);
+    ba_dump_schur_kernel<<<nprob, 256, 0, ctx->stream>>>(dp, S_out, rhs_out, info);
     ALVA_LAUNCH_CHECK(ctx);
     return 0;
 }

@@ -80,6 +80,8 @@ _OPTIONAL = {
     "alva_k_ba_local": [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_double, C.c_double,
                         _i32, _vp, _vp],
     "alva_k_ba_linearize": [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_double, _vp, _vp, _vp, _vp, _vp],
+    "alva_k_ba_schur_dump": [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_double, _i32, _vp, _vp,
+                             _vp],
 }
 
 
@@ -293,3 +295,10 @@ class Context:
         self._chk(self.L.alva_k_ba_linearize(self.h, nkf, nlm, nobs, _ptr(calib), _ptr(poses), _ptr(invd), _ptr(anch_kf),
                                              _ptr(anch_uv), _ptr(obs_kf), _ptr(obs_lm), _ptr(obs_uv), huber, _ptr(res),
                                              _ptr(Ja), _ptr(Jp), _ptr(Jd), _ptr(cost)))
+
+    def ba_schur_dump(self, nprob, nkf, nlm, nobs, calib, poses, pose_const, invd, anch_kf, anch_uv, obs_kf, obs_lm, obs_uv,
+                      huber, atomic, S, rhs, info):
+        """test hook: the first LM iteration's reduced camera system -- see alva_k_ba_schur_dump"""
+        self._chk(self.L.alva_k_ba_schur_dump(self.h, nprob, nkf, nlm, nobs, _ptr(calib), _ptr(poses), _ptr(pose_const),
+                                              _ptr(invd), _ptr(anch_kf), _ptr(anch_uv), _ptr(obs_kf), _ptr(obs_lm), _ptr(obs_uv),
+                                              huber, int(atomic), _ptr(S), _ptr(rhs), _ptr(info)))

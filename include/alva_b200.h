@@ -351,6 +351,15 @@ int alva_k_ba_linearize(alva_ctx*, int nkf, int nlm, int nobs, const double* cal
                         const double* obs_uv, double huber_delta, double* res, double* Ja, double* Jp, double* Jd,
                         double* cost_per_obs);
 
+/* Test hook: the reduced camera system of alva_k_ba_solve's first Levenberg-Marquardt iteration (the input point's
+ * linearisation, Jacobi scaling and LM diagonal; inputs as alva_k_ba_solve, not modified), assembled by the path the solve takes
+ * (atomic = 0) or by the atomic per-landmark path (atomic = 1).  S_out [nprob][128][128] (rows / columns past the width are 0),
+ * rhs_out [nprob][128], info [nprob][2] = {reduced-system width, 1 if the gather path assembled it}.  Needs ba_dense_schur off. */
+int alva_k_ba_schur_dump(alva_ctx*, int nprob, int nkf, int nlm, int nobs, const double* calib, const double* poses,
+                         const uint8_t* pose_const, const double* invd, const int32_t* anch_kf, const double* anch_uv,
+                         const int32_t* obs_kf, const int32_t* obs_lm, const double* obs_uv, double huber_delta, int atomic,
+                         double* S_out, double* rhs_out, double* info);
+
 /* ---- the whole per-frame hot path as one object ------------------------------------------------
  * A batch of frames goes gray + pyramid + FAST -> retainBest -> ORB -> Hamming 2-NN vs the local map -> local BA on
  * the step's keyframes, every intermediate resident in HBM, no host synchronisation inside a step

@@ -5,7 +5,8 @@
                   frame stages, and without BA (kf_interval 0): if the no-BA step is close to the full one, BA does not bound it
   chain           one standalone 13-problem alva_k_ba_solve, CUDA events (as tools/gpu_ba_bench.py)
   kernels         the same solve under torch.profiler (CUDA activities), in a pass of its own: each ba_* kernel's total time
-                  and call count per solve
+                  and call count per solve, and its duration per launch in launch order (us_per_launch)
+  dense_schur     chain and kernels again with alva_set_option("ba_dense_schur", 1): the Schur term as an FP64 tensor-core SYRK
   card            name and power limit, read in the same run
 
     python tools/gpu_ba_chain_profile.py --out profiles/ba_chain_h100.json
@@ -104,45 +105,68 @@ def main():
         e1.record()
         return e0, e1
 
-    for _ in range(3):
-        solve()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(args.reps):
-        l0 = ctx.launches
-        e0, e1 = solve()
-        torch.cuda.synchronize()
-        ts.append(e0.elapsed_time(e1))
-        launches = ctx.launches - l0
-    s = summ.cpu().numpy()[0]
-    res["chain_ms"] = {"median": float(np.median(ts)), "min": float(np.min(ts)), "max": float(np.max(ts)), "reps": args.reps,
-                       "launches_per_solve_incl_summary": int(launches),
-                       "summary_problem0": {"initial_cost": float(s[0]), "final_cost": float(s[1]), "n_success": int(s[2]),
-                                            "n_iter": int(s[3]), "term": int(s[4])}}
-
-    # ---- per-kernel times, torch.profiler in a pass of its own
-    nprof = 10
-    from torch.profiler import profile, ProfilerActivity
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for _ in range(nprof):
+    def timed(dense):
+        ctx.L.alva_set_option(b"ba_dense_schur", dense)
+        for _ in range(3):
             solve()
         torch.cuda.synchronize()
-    kern = {}
-    for ev in prof.key_averages():
-        name = kernel_name(ev.key)
-        if not name:
-            continue
-        t = getattr(ev, "device_time_total", None)
-        if t is None:
-            t = ev.cuda_time_total
-        k = kern.setdefault(name, {"us_per_solve": 0.0, "calls_per_solve": 0.0})
-        k["us_per_solve"] += t / nprof
-        k["calls_per_solve"] += ev.count / nprof
-    for k in kern.values():
-        k["us_per_call"] = k["us_per_solve"] / k["calls_per_solve"] if k["calls_per_solve"] else 0.0
-    res["kernels"] = dict(sorted(kern.items(), key=lambda kv: -kv[1]["us_per_solve"]))
-    res["kernels_total_us_per_solve"] = sum(k["us_per_solve"] for k in kern.values())
-    res["kernels_note"] = f"torch.profiler, CUDA activities, {nprof} solves after the timed pass; times are kernel durations"
+        ts = []
+        for _ in range(args.reps):
+            l0 = ctx.launches
+            e0, e1 = solve()
+            torch.cuda.synchronize()
+            ts.append(e0.elapsed_time(e1))
+            launches = ctx.launches - l0
+        s = summ.cpu().numpy()[0]
+        out = {"median": float(np.median(ts)), "min": float(np.min(ts)), "max": float(np.max(ts)), "reps": args.reps,
+               "launches_per_solve_incl_summary": int(launches),
+               "summary_problem0": {"initial_cost": float(s[0]), "final_cost": float(s[1]), "n_success": int(s[2]),
+                                    "n_iter": int(s[3]), "term": int(s[4])}}
+        ctx.L.alva_set_option(b"ba_dense_schur", 0)
+        return out
+
+    # ---- per-kernel times, torch.profiler in a pass of its own: totals per solve, and every launch in launch order (a launch
+    # whose problems are all finished returns at once, so the active ones stand apart)
+    nprof = 10
+
+    def profiled(dense):
+        from torch.profiler import profile, ProfilerActivity
+        from torch.autograd import DeviceType
+        ctx.L.alva_set_option(b"ba_dense_schur", dense)
+        for _ in range(3):
+            solve()
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(nprof):
+                solve()
+            torch.cuda.synchronize()
+        ctx.L.alva_set_option(b"ba_dense_schur", 0)
+        evs = sorted((e for e in prof.events() if e.device_type == DeviceType.CUDA and kernel_name(e.name)),
+                     key=lambda e: e.time_range.start)
+        solves = []   # per solve: kernel -> [us of launch 1, 2, ...]
+        for e in evs:
+            name = kernel_name(e.name)
+            if name == "ba_setup_kernel":
+                solves.append({})
+            if solves:
+                solves[-1].setdefault(name, []).append(e.time_range.elapsed_us())
+        assert len(solves) == nprof, len(solves)
+        kern, launch = {}, {}
+        for name in solves[0]:
+            per = np.array([sv[name] for sv in solves], dtype=np.float64)   # [solve][launch]
+            kern[name] = {"us_per_solve": float(per.sum(1).mean()), "calls_per_solve": per.shape[1],
+                          "us_per_call": float(per.mean())}
+            launch[name] = [round(float(v), 2) for v in per.mean(0)]
+        kern = dict(sorted(kern.items(), key=lambda kv: -kv[1]["us_per_solve"]))
+        return {"kernels": kern, "kernels_total_us_per_solve": sum(k["us_per_solve"] for k in kern.values()),
+                "us_per_launch": {k: launch[k] for k in kern},
+                "kernels_note": f"torch.profiler, CUDA activities, {nprof} solves after the timed pass; times are kernel durations, "
+                                "us_per_launch in launch order, averaged over the solves"}
+
+    res["chain_ms"] = timed(0)
+    res.update(profiled(0))
+    # the same with the Schur term as an FP64 tensor-core SYRK (alva_set_option("ba_dense_schur", 1))
+    res["dense_schur"] = {"chain_ms": timed(1), **profiled(1)}
     ctx.close()
 
     txt = json.dumps(res, indent=1)
