@@ -19,6 +19,7 @@ def _bind():
     L.alva_system_reset.argtypes = [_vp]
     L.alva_system_set_clahe.argtypes = [_vp, _i32, _f64, _i32]
     L.alva_system_set_distortion.argtypes = [_vp] + [_f64] * 4
+    L.alva_system_set_preset.argtypes = [_vp, _i32]
     L.alva_system_num_matched.argtypes = [_vp]
     L.alva_system_configure.argtypes = [_vp, _i32, _i32] + [_f64] * 8
     L.alva_system_find_camera_pose.argtypes = [_vp, _vp, _vp]
@@ -130,6 +131,20 @@ class System:
         rc = self.L.alva_system_set_clahe(self.h, 1 if enabled else 0, float(clip_limit), int(tile_size))
         if rc != 0:
             raise AlvaError(f"alva_system_set_clahe -> {rc}: {self.L.alva_last_error().decode()}")
+
+    PRESETS = {"default": 0, "fast": 1, "average": 2, "accurate": 3}   # ALVA_PRESET_* (include/alva_b200.h)
+
+    def set_preset(self, name):
+        """The reference's tuned configurations: "default" (what configuring sets: 40-px grid cells, P3P on every frame,
+        keyframe filtering ratio 0.95, CLAHE off), "fast" (50 px, 0.9), "average" (45 px, 0.9, PnP from the motion prior
+        instead of P3P) or "accurate" (35 px, PnP from the prior, CLAHE on with clip 3 and 50-px tiles).  Resets the tracker
+        and the map; the next frame starts under the preset.  Survives reset(); set_clahe() afterwards overrides its CLAHE
+        setting; the lens model is kept."""
+        if name not in self.PRESETS:
+            raise ValueError(f"unknown preset {name!r}: one of {sorted(self.PRESETS)}")
+        rc = self.L.alva_system_set_preset(self.h, self.PRESETS[name])
+        if rc != 0:
+            raise AlvaError(f"alva_system_set_preset -> {rc}: {self.L.alva_last_error().decode()}")
 
     def set_distortion(self, k1, k2, p1, p2):
         """OpenCV's radial-tangential lens model (the reference's configure(..., k1, k2, p1, p2)): keypoints are undistorted,

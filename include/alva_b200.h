@@ -433,6 +433,22 @@ int  alva_system_set_clahe(alva_system*, int enabled, double clip_limit, int til
  * reset() does; the next frame starts under the new model.  All zero = the pinhole camera.  configure clears it, reset keeps it.
  * ALVA_E_STATE before configure; ALVA_E_INVALID for a null handle or a non-finite coefficient. */
 int  alva_system_set_distortion(alva_system*, double k1, double k2, double p1, double p2);
+/* The reference's three tuned configurations (state.hpp:9-17), and DEFAULT = what configure sets (system.cpp:15-19):
+ *              grid cell  CLAHE (clip 3, tile 50)  keyframe filtering ratio  P3P on every tracked frame
+ *   DEFAULT    40 px      off                      0.95                      yes
+ *   FAST       50 px      off                      0.9                       yes
+ *   AVERAGE    45 px      off                      0.9                       no: PnP from the motion prior, P3P on the next frame if it fails
+ *   ACCURATE   35 px      on                       0.95                      no
+ * The cell size sets the detector grid, the keypoint budget ceil(w / cell) * ceil(h / cell), the local-map size, the keyframe
+ * rules and the grid the local-map matcher searches.  It resets the tracker and the map as reset() does (the frame grid
+ * changes); the next frame starts under the new preset.  It sets the CLAHE switch from the table: a later
+ * alva_system_set_clahe overrides it.  configure returns the handle to DEFAULT, reset keeps the preset, the lens model is left
+ * alone.  ALVA_E_STATE before configure; ALVA_E_INVALID for a null handle or an unknown preset. */
+#define ALVA_PRESET_DEFAULT  0
+#define ALVA_PRESET_FAST     1
+#define ALVA_PRESET_AVERAGE  2
+#define ALVA_PRESET_ACCURATE 3
+int  alva_system_set_preset(alva_system*, int preset);
 int  alva_system_find_camera_pose(alva_system*, const uint8_t* rgba, float* pose16);
 /* the same with the frame's time stamp (milliseconds) supplied by the caller instead of read from the system clock
  * (system.cpp:114): deterministic replays, and hosts that deliver frames faster than real time (two frames inside one

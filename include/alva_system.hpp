@@ -29,6 +29,8 @@ public:
         status_ = alva_system_configure(h_, imageWidth, imageHeight, fx, fy, cx, cy, k1, k2, p1, p2);
     }
     void reset() { alva_system_reset(h_); }
+    // not in the reference's class: its FAST / AVERAGE / ACCURATE presets (ALVA_PRESET_*, alva_b200.h); 0 or an ALVA_E_* code
+    int setPreset(int preset) { return alva_system_set_preset(h_, preset); }
 
     // ---- the reference's wasm32 signatures
     int findCameraPose(int imageRGBADataPtr, int posePtr) { return findCameraPose(ptr<const uint8_t>(imageRGBADataPtr), ptr<float>(posePtr)); }
