@@ -173,7 +173,9 @@ __global__ void __launch_bounds__(WPC * 32, 3) knn2_blockpair_kernel(const uint8
     if (r == rank) return;
     const uint8_t* lb = gathered + ((size_t)rank * K + e) * block_bytes;
     const uint8_t* rb = gathered + ((size_t)r * K + e) * block_bytes;
-    const int nq = min(reinterpret_cast<const int32_t*>(lb)[4], n_max), nt = min(reinterpret_cast<const int32_t*>(rb)[4], n_max);
+    // header counts come from other ranks: clamped to [0, n_max] (a negative train count would step the tail before the array)
+    const int nq = min(max(reinterpret_cast<const int32_t*>(lb)[4], 0), n_max);
+    const int nt = min(max(reinterpret_cast<const int32_t*>(rb)[4], 0), n_max);
     const int q0 = (blockIdx.x * WPC + warp) * QPW;
     if (q0 >= nq) return;
     const uint4* q = reinterpret_cast<const uint4*>(lb + hdr_bytes + (size_t)n_max * 8);

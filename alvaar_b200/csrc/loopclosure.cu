@@ -1,7 +1,8 @@
 // loopclosure.cu -- cross-stream loop-closure detection over exchanged keyframe blocks (SURVEY 8e / 8f.4).
 //
 // The reference has no loop closure and no multi-stream mode (iBoW-LCD is vendored but never linked), so nothing here has a
-// reference behaviour to match: PARITY UNPINNED for this stage -- it is validated by determinism and planted revisits
+// reference behaviour to match: PARITY UNPINNED for this stage -- it is validated stage by stage against a host model of what it
+// computes (tests/lc_util.py, tests/test_gpu_loopclosure_model.py) and end to end by determinism and planted revisits
 // (tests/test_gpu_loopclosure.py).  Capability model (not code): src/libs/ibow_lcd/src/lcdetector.cc -- candidate scoring,
 // consecutive-detection ("island") consistency, geometric verification before a loop is reported.
 //
@@ -29,7 +30,10 @@ int alva_knn2_blockpair_launch(alva_ctx* ctx, const uint8_t* gathered, size_t bl
 namespace {
 
 constexpr int HDR = ALVA_LC_HEADER_BYTES;
-constexpr int PAIR_CAP = 512;   // putative matches kept per keyframe pair (more than enough for RANSAC)
+constexpr int PAIR_CAP = ALVA_LC_PAIR_CAP;   // putative matches kept per keyframe pair (more than enough for RANSAC)
+
+// a header count, written by another rank: live entries in [0, n_max]
+__device__ __forceinline__ int live_count(int count, int n_max) { return min(max(count, 0), n_max); }
 
 // header words: 0 magic, 1 version, 2 stream id, 3 keyframe sequence number, 4 count, 5 n_max, 6..9 fx fy cx cy (float)
 __global__ void lc_pack_kernel(const uint8_t* __restrict__ desc, const float* __restrict__ pts, const int32_t* __restrict__ counts,
@@ -37,7 +41,7 @@ __global__ void lc_pack_kernel(const uint8_t* __restrict__ desc, const float* __
                                float cx, float cy, uint8_t* __restrict__ send, size_t block_bytes) {
     const int e = blockIdx.y;
     const int f = kf_frames[e];
-    const int n = min(min(counts[f], cap), n_max);
+    const int n = live_count(min(counts[f], cap), n_max);
     uint8_t* blk = send + (size_t)e * block_bytes;
     if (blockIdx.x == 0 && threadIdx.x < 16) {
         int32_t* h = reinterpret_cast<int32_t*>(blk);
@@ -91,7 +95,7 @@ __global__ void __launch_bounds__(256) lc_score_kernel(const uint8_t* __restrict
     const float* lf = reinterpret_cast<const float*>(lb);
     const float* rf = reinterpret_cast<const float*>(rb);
     const bool valid = lh[0] == ALVA_LC_MAGIC && rh[0] == ALVA_LC_MAGIC && lh[1] == ALVA_LC_VERSION && rh[1] == ALVA_LC_VERSION;
-    const int nq = valid ? min(lh[4], n_max) : 0;
+    const int nq = valid ? live_count(lh[4], n_max) : 0;
     const float2* lpx = reinterpret_cast<const float2*>(lb + HDR);
     const float2* rpx = reinterpret_cast<const float2*>(rb + HDR);
     const int4* my = nn + (size_t)p * n_max;
@@ -146,7 +150,7 @@ __global__ void lc_collect_kernel(const uint8_t* __restrict__ gathered, size_t b
     const int e = p / world, r = p - e * world;
     const int32_t* rh = reinterpret_cast<const int32_t*>(gathered + ((size_t)r * K + e) * block_bytes);
     const int32_t* lh = reinterpret_cast<const int32_t*>(gathered + ((size_t)rank * K + e) * block_bytes);
-    const int nq = lh[0] == ALVA_LC_MAGIC ? min(lh[4], n_max) : 0;
+    const int nq = lh[0] == ALVA_LC_MAGIC ? live_count(lh[4], n_max) : 0;
     const bool enough = r != rank && nmatch[p] >= max(min_matches, nq / 8);
     double* o = out + (size_t)p * 16;
     o[0] = nmatch[p]; o[1] = e == K - 1 ? info[4 * p] : (enough ? 2.0 : 0.0); o[2] = info[4 * p + 1]; o[3] = rh[3];
@@ -320,5 +324,18 @@ extern "C" int alva_lc_last_scores(alva_lc* lc, double* out) { AlvaDeviceGuard g
     std::vector<double> h((size_t)lc->npair * 16);
     ALVA_CUDA(cudaMemcpy(h.data(), lc->res_dev, h.size() * 8, cudaMemcpyDeviceToHost));
     for (int p = 0; p < lc->npair; p++) for (int i = 0; i < 4; i++) out[4 * p + i] = h[(size_t)p * 16 + i];
+    return 0;
+}
+
+// the 2-NN lists, geometric-check sizes and bearing vectors of the last step (tests / diagnostics); any output may be NULL
+extern "C" int alva_lc_last_matches(alva_lc* lc, int32_t* nn, int32_t* npair, double* bv_local, double* bv_remote) {
+    AlvaDeviceGuard guard__(lc ? lc->ctx : nullptr);
+    if (!lc) return ALVA_E_INVALID;
+    const size_t np = lc->npair;
+    ALVA_CUDA(cudaStreamSynchronize(lc->ctx->stream));
+    if (nn) ALVA_CUDA(cudaMemcpy(nn, lc->nn, np * lc->cfg.n_max * 16, cudaMemcpyDeviceToHost));
+    if (npair) ALVA_CUDA(cudaMemcpy(npair, lc->npairs, np * 4, cudaMemcpyDeviceToHost));
+    if (bv_local) ALVA_CUDA(cudaMemcpy(bv_local, lc->bvl, np * PAIR_CAP * 24, cudaMemcpyDeviceToHost));
+    if (bv_remote) ALVA_CUDA(cudaMemcpy(bv_remote, lc->bvr, np * PAIR_CAP * 24, cudaMemcpyDeviceToHost));
     return 0;
 }

@@ -6,7 +6,7 @@ import numpy as np
 
 from .lib import AlvaError, lib
 
-MAGIC, VERSION, HEADER_BYTES = 0x464B4C41, 1, 64
+MAGIC, VERSION, HEADER_BYTES, PAIR_CAP = 0x464B4C41, 1, 64, 512
 
 
 class LcConfig(C.Structure):
@@ -100,3 +100,15 @@ class LoopClosure:
         out = np.zeros((self.K, self.world, 4))
         self._chk(self.L.alva_lc_last_scores(self.h, out.ctypes.data_as(C.c_void_p)))
         return out
+
+    def last_matches(self):
+        """internal state of the last step (tests / diagnostics): nn [K, world, n_max, 4] = (idx0, dist0, idx1, dist1) of the 2-NN, -1
+        where there is none, defined below the local live count; npair [K, world] = correspondences of the geometric check;
+        bv_local, bv_remote [K, world, PAIR_CAP, 3] = bearing vectors of the putative matches in local-index order"""
+        nn = np.zeros((self.K, self.world, self.n_max, 4), np.int32)
+        npair = np.zeros((self.K, self.world), np.int32)
+        bvl = np.zeros((self.K, self.world, PAIR_CAP, 3))
+        bvr = np.zeros((self.K, self.world, PAIR_CAP, 3))
+        self.L.alva_lc_last_matches.argtypes = [C.c_void_p] * 5
+        self._chk(self.L.alva_lc_last_matches(self.h, *(a.ctypes.data_as(C.c_void_p) for a in (nn, npair, bvl, bvr))))
+        return nn, npair, bvl, bvr

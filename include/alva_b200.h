@@ -481,7 +481,8 @@ int  alva_system_unpin_buffer(alva_system*, void* host_ptr);
  * planted revisits).  KEYFRAME BLOCK wire format (what one rank contributes per new keyframe to the NCCL all-gather;
  * little-endian, fixed size so that the exchange has static shapes):
  *     offset 0    int32 magic = ALVA_LC_MAGIC ('ALKF'), int32 version = ALVA_LC_VERSION, int32 stream id (rank), int32 keyframe
- *                 sequence number, int32 count (live entries, <= n_max), int32 n_max, float32 fx, fy, cx, cy, 6 x int32 reserved (0)
+ *                 sequence number, int32 count (live entries, <= n_max; a reader clamps it to [0, n_max]), int32 n_max,
+ *                 float32 fx, fy, cx, cy, 6 x int32 reserved (0)
  *     offset 64   float32 px[n_max][2]      pixel position of keypoint i (entries >= count are 0)
  *     then        uint8   desc[n_max][32]   its 256-bit ORB descriptor
  * alva_lc_block_bytes(n_max) = 64 + 40 * n_max.  A step's exchange is [world][kf_per_step] such blocks.
@@ -497,6 +498,7 @@ int  alva_system_unpin_buffer(alva_system*, void* host_ptr);
 #define ALVA_LC_MAGIC        0x464B4C41   /* "ALKF" */
 #define ALVA_LC_VERSION      1
 #define ALVA_LC_HEADER_BYTES 64
+#define ALVA_LC_PAIR_CAP     512          /* putative matches kept per keyframe pair (the first ones in local-index order) */
 typedef struct alva_lc alva_lc;
 typedef struct {
     int32_t n_max, kf_per_step, world, rank;
@@ -527,6 +529,12 @@ int      alva_lc_poll(alva_lc*, alva_lc_event* out, int cap, int wait);
 int      alva_lc_inflight(const alva_lc*);
 /* diagnostics: per keyframe pair of the last step, out [kf_per_step][world][4] = {matches, RANSAC success, inliers, remote keyframe} */
 int      alva_lc_last_scores(alva_lc*, double* out);
+/* tests / diagnostics: the internal state of the last step.  nn [kf_per_step][world][n_max][4] = {idx0, dist0, idx1, dist1} of the
+ * Hamming 2-NN (-1 where there is none; only rows below the local keyframe's live count are defined), npair [kf_per_step][world] =
+ * correspondences handed to the geometric check, bv_local / bv_remote [kf_per_step][world][ALVA_LC_PAIR_CAP][3] = the bearing
+ * vectors of the putative matches in local-index order (rows below min(matches, ALVA_LC_PAIR_CAP) are defined).  Any output
+ * may be NULL. */
+int      alva_lc_last_matches(alva_lc*, int32_t* nn, int32_t* npair, double* bv_local, double* bv_remote);
 
 /* N independent camera streams in one call (SURVEY 8e: streams are independent, System holds all state): handles[i]
  * processes the frame rgba[i] with time stamp t_ms[i] (t_ms NULL = the system clock).  poses16 [n][16], status [n] (the value
