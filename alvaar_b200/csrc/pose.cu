@@ -19,6 +19,8 @@
 //   * all hypotheses of a problem are solved at once (thread per draw), kept in the reference's order;
 //   * one CTA per (hypothesis, problem) computes the N squared distances and takes the median by a bitonic sort in
 //     shared memory; a last kernel picks the first strict minimum, classifies inliers and checks orthogonality;
+//   * P3P-RANSAC (alva_k_p3p_ransac, System's relocalisation) runs the same hypotheses kernel, counts each hypothesis'
+//     inliers instead of sorting, and the last kernel picks the first strict maximum;
 //   * the PnP refinement is one CTA per problem with every LM decision on the device (fixed-order reductions: the result
 //     is bit-reproducible run to run).
 #include "alva_common.cuh"
@@ -303,7 +305,31 @@ __global__ void __launch_bounds__(MED_THREADS) p3p_median_kernel(const LmedsPara
     }
 }
 
+// ------------------------------------------------------------------ kernel B': inlier count per hypothesis (RANSAC)
+// one CTA per (hypothesis, problem): pen[k] = #points with bearing distance <= threshold under hypothesis k
+__global__ void __launch_bounds__(MED_THREADS) p3p_inlier_count_kernel(const LmedsParams P) {
+    __shared__ int cnt[MED_THREADS];
+    const int prob = blockIdx.y, hy = blockIdx.x, tid = threadIdx.x;
+    if (hy >= P.nhyp[2 * prob]) return;
+    const int n = P.counts ? min(P.counts[prob], P.cap) : P.cap;
+    const double* bvs = P.bvs + (size_t)prob * P.cap * 3;
+    const double* wpts = P.wpts + (size_t)prob * P.cap * 3;
+    double T[12];
+    const double* Tg = P.hyp + ((size_t)prob * P.max_iter + hy) * 12;
+#pragma unroll
+    for (int i = 0; i < 12; i++) T[i] = Tg[i];
+    int mine = 0;
+    for (int i = tid; i < n; i += MED_THREADS) mine += bearing_dist(T, wpts + 3 * i, bvs + 3 * i) <= P.threshold;
+    cnt[tid] = mine;
+    __syncthreads();
+    for (int s = MED_THREADS / 2; s > 0; s >>= 1) { if (tid < s) cnt[tid] += cnt[tid + s]; __syncthreads(); }
+    if (tid == 0) P.pen[(size_t)prob * P.max_iter + hy] = (double)cnt[0];
+}
+
 // ------------------------------------------------------------------ kernel C: best model, inliers, checks
+// LMedS (RANSAC = false): the first strict minimum of the median; RANSAC: the first strict maximum of the inlier count (a
+// hypothesis without inliers is never selected).  info[2] = the best median (LMedS) / the selected hypothesis' index (RANSAC).
+template <bool RANSAC>
 __global__ void __launch_bounds__(256) p3p_select_kernel(const LmedsParams P) {
     __shared__ int s_best;
     __shared__ double s_pen;
@@ -313,13 +339,13 @@ __global__ void __launch_bounds__(256) p3p_select_kernel(const LmedsParams P) {
     uint8_t* outl = P.outlier + (size_t)prob * P.cap;
     double* info = P.info ? P.info + 4 * prob : nullptr;
     if (tid == 0) {
-        double best = DBL_MAX;
+        double best = RANSAC ? 0.0 : DBL_MAX;
         int bi = -1;
         for (int k = 0; k < nh; k++) {
             const double v = P.pen[(size_t)prob * P.max_iter + k];
-            if (v < best) { best = v; bi = k; }
+            if (RANSAC ? v > best : v < best) { best = v; bi = k; }
         }
-        s_best = bi; s_pen = best;
+        s_best = bi; s_pen = RANSAC ? (double)bi : best;
     }
     __syncthreads();
     const int bi = s_best;
@@ -815,6 +841,19 @@ static void make_rnd_table(uint32_t seed, int n, std::vector<int32_t>& out) {
     for (int i = 0; i < n; i++) out[i] = dist(alg);
 }
 
+// the sampler table depends only on (seed, length) and a longer table starts with the shorter one: kept on the device across
+// calls (System draws it every frame) and regrown only when a caller needs more of it or another seed
+static int p3p_rnd_table(alva_ctx* ctx, uint32_t seed, int len) {
+    if (ctx->p3p_tab && ctx->p3p_tab_len >= len && ctx->p3p_tab_seed == seed) return 0;
+    std::vector<int32_t> host_tab;
+    make_rnd_table(seed, len, host_tab);
+    if (ctx->p3p_tab) { ALVA_CUDA(cudaStreamSynchronize(ctx->stream)); ALVA_CUDA(cudaFree(ctx->p3p_tab)); ctx->p3p_tab = nullptr; }
+    ALVA_CUDA(cudaMalloc(&ctx->p3p_tab, (size_t)len * 4));
+    ALVA_CUDA(cudaMemcpy(ctx->p3p_tab, host_tab.data(), (size_t)len * 4, cudaMemcpyHostToDevice));
+    ctx->p3p_tab_len = len; ctx->p3p_tab_seed = seed;
+    return 0;
+}
+
 extern "C" int alva_k_p3p_lmeds(alva_ctx* ctx, int nprob, int cap, const double* bvs, const double* wpts, const int32_t* counts,
                                 int max_iter, float err_px, float fx, float fy, uint32_t seed, double* Twc_out,
                                 uint8_t* outlier, double* info) { AlvaDeviceGuard guard__(ctx);
@@ -838,16 +877,8 @@ extern "C" int alva_k_p3p_lmeds(alva_ctx* ctx, int nprob, int cap, const double*
     int32_t* tab = (int32_t*)(ws + hyp_b + pen_b);
     P.rnd = tab; P.nhyp = (int32_t*)(ws + hyp_b + pen_b + tab_b);
     P.Twc = Twc_out; P.outlier = outlier; P.info = info;
-    // the sampler table depends only on (seed, length): kept on the device across calls (System draws it every frame)
-    if (!ctx->p3p_tab || ctx->p3p_tab_len != P.table_len || ctx->p3p_tab_seed != seed) {
-        std::vector<int32_t> host_tab;
-        make_rnd_table(seed, P.table_len, host_tab);
-        if (ctx->p3p_tab) { ALVA_CUDA(cudaStreamSynchronize(ctx->stream)); ALVA_CUDA(cudaFree(ctx->p3p_tab)); ctx->p3p_tab = nullptr; }
-        ALVA_CUDA(cudaMalloc(&ctx->p3p_tab, (size_t)P.table_len * 4));
-        ALVA_CUDA(cudaMemcpy(ctx->p3p_tab, host_tab.data(), (size_t)P.table_len * 4, cudaMemcpyHostToDevice));
-        ctx->p3p_tab_len = P.table_len; ctx->p3p_tab_seed = seed;
-    }
     (void)tab;
+    if (int e = p3p_rnd_table(ctx, seed, P.table_len)) return e;
     P.rnd = (const int32_t*)ctx->p3p_tab;
     p3p_hypotheses_kernel<<<nprob, HYP_THREADS, (size_t)cap * sizeof(int), ctx->stream>>>(P);
     ALVA_LAUNCH_CHECK(ctx);
@@ -855,7 +886,40 @@ extern "C" int alva_k_p3p_lmeds(alva_ctx* ctx, int nprob, int cap, const double*
     while (m < cap) m <<= 1;
     p3p_median_kernel<<<dim3(max_iter, nprob), MED_THREADS, (size_t)m * 8, ctx->stream>>>(P, m);
     ALVA_LAUNCH_CHECK(ctx);
-    p3p_select_kernel<<<nprob, 256, 0, ctx->stream>>>(P);
+    p3p_select_kernel<false><<<nprob, 256, 0, ctx->stream>>>(P);
+    ALVA_LAUNCH_CHECK(ctx);
+    return 0;
+}
+
+// P3P-RANSAC: the sampler and hypotheses of alva_k_p3p_lmeds (the same kernel: the same seed gives the same hypotheses),
+// each scored by its inlier count at the same threshold; the first strict maximum is the model
+extern "C" int alva_k_p3p_ransac(alva_ctx* ctx, int nprob, int cap, const double* bvs, const double* wpts, const int32_t* counts,
+                                 int max_iter, float err_px, float fx, float fy, uint32_t seed, double* Twc_out,
+                                 uint8_t* outlier, double* info) { AlvaDeviceGuard guard__(ctx);
+    if (!ctx || !bvs || !wpts || !Twc_out || !outlier || nprob < 1 || cap < 1 || max_iter < 1 || max_iter > 1024) {
+        alva_set_error("alva_k_p3p_ransac: bad argument");
+        return ALVA_E_INVALID;
+    }
+    if (cap > 8192) { alva_set_error("alva_k_p3p_ransac: at most 8192 points per problem (got %d)", cap); return ALVA_E_INVALID; }
+    float focal = fx + fy;
+    focal = (float)(focal / 2.);
+    LmedsParams P{};
+    P.threshold = 1.0 - cosf(atanf(err_px / focal));
+    P.bvs = bvs; P.wpts = wpts; P.counts = counts; P.cap = cap; P.max_iter = max_iter; P.max_skip = max_iter * 10;
+    P.table_len = 4 * (max_iter + P.max_skip + HYP_THREADS);
+    const size_t hyp_b = (size_t)nprob * max_iter * 12 * sizeof(double), pen_b = (size_t)nprob * max_iter * sizeof(double);
+    const size_t nh_b = ((size_t)nprob * 8 + 255) & ~(size_t)255;
+    uint8_t* ws = (uint8_t*)alva_scratch(ctx, hyp_b + pen_b + nh_b + 1024);
+    if (!ws) return ALVA_E_CUDA;
+    P.hyp = (double*)ws; P.pen = (double*)(ws + hyp_b); P.nhyp = (int32_t*)(ws + hyp_b + pen_b);
+    P.Twc = Twc_out; P.outlier = outlier; P.info = info;
+    if (int e = p3p_rnd_table(ctx, seed, P.table_len)) return e;
+    P.rnd = (const int32_t*)ctx->p3p_tab;
+    p3p_hypotheses_kernel<<<nprob, HYP_THREADS, (size_t)cap * sizeof(int), ctx->stream>>>(P);
+    ALVA_LAUNCH_CHECK(ctx);
+    p3p_inlier_count_kernel<<<dim3(max_iter, nprob), MED_THREADS, 0, ctx->stream>>>(P);
+    ALVA_LAUNCH_CHECK(ctx);
+    p3p_select_kernel<true><<<nprob, 256, 0, ctx->stream>>>(P);
     ALVA_LAUNCH_CHECK(ctx);
     return 0;
 }
@@ -882,6 +946,18 @@ int alva_pose_chain_launch(alva_ctx* ctx, int n, int cap, const double* bvs, con
                            int32_t* n2, double* pose7, uint8_t* o2, double* summ, double huber, double chi2) {
     if (int e = alva_k_p3p_lmeds(ctx, 1, n, bvs, X, nullptr, 100, 3.0f, fx, fy, seed, T12, o1, info)) return e;
     pnp_from_p3p_kernel<<<1, 256, 0, ctx->stream>>>(cap, nullptr, n, T12, o1, uv, X, uv2, X2, n2, pose7);
+    ALVA_LAUNCH_CHECK(ctx);
+    return alva_k_pnp(ctx, 1, cap, K4, uv2, X2, n2, pose7, huber, chi2, 5, 1, 1, o2, summ);
+}
+
+// internal (system.cu): the pose of a relocalised frame -- P3P-RANSAC (max_iter hypotheses) on the counts[0] correspondences
+// alva_reloc_compact_launch wrote, the same hand-over as alva_pose_chain_launch, PnP on the RANSAC inliers; no host
+// synchronisation.  Buffers as alva_pose_chain_launch, every point list [cap].
+int alva_reloc_pose_launch(alva_ctx* ctx, int cap, const int32_t* counts, const double* bvs, const double* X, const double* uv,
+                           const double* K4, float fx, float fy, uint32_t seed, int max_iter, double* T12, double* info, uint8_t* o1,
+                           double* uv2, double* X2, int32_t* n2, double* pose7, uint8_t* o2, double* summ, double huber, double chi2) {
+    if (int e = alva_k_p3p_ransac(ctx, 1, cap, bvs, X, counts, max_iter, 3.0f, fx, fy, seed, T12, o1, info)) return e;
+    pnp_from_p3p_kernel<<<1, 256, 0, ctx->stream>>>(cap, counts, 0, T12, o1, uv, X, uv2, X2, n2, pose7);
     ALVA_LAUNCH_CHECK(ctx);
     return alva_k_pnp(ctx, 1, cap, K4, uv2, X2, n2, pose7, huber, chi2, 5, 1, 1, o2, summ);
 }

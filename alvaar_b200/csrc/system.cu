@@ -21,6 +21,8 @@
 //   triangulate  new map points at keyframes                      alva_k_triangulate                (multi_view_geometry.cpp:12-22)
 //   match_to_map local map -> keyframe matching                   alva_k_match_to_map               (mapper.cpp:354-587)
 //   ba_local     local bundle adjustment, both solves + flags     alva_k_ba_local                   (optimizer.cpp:251-359)
+//   relocalise   a lost frame against the frozen map              alva_k_hamming_knn2_grouped, match rules, alva_k_p3p_ransac, alva_k_pnp
+//                (not in the reference: alva_system_set_relocalisation)
 // There is no CPU fallback: configure() fails without an sm_90 (H100) device.  Lens distortion: the JS shim always passes zeros
 // (system.js:84-141) and configure() rejects non-zero coefficients; setDistortion() (alva_system_set_distortion) sets them on a
 // configured System.  With distortion on, klt and detect undistort the points they return with alva_k_undistort_points on the
@@ -42,6 +44,12 @@ int alva_undistort_points_launch(alva_ctx* ctx, const float* px, const int32_t* 
 int alva_pose_chain_launch(alva_ctx* ctx, int n, int cap, const double* bvs, const double* X, const double* uv, const double* K4,
                            float fx, float fy, uint32_t seed, double* T12, double* info, uint8_t* o1, double* uv2, double* X2,
                            int32_t* n2, double* pose7, uint8_t* o2, double* summ, double huber, double chi2);
+int alva_reloc_compact_launch(alva_ctx* ctx, const int32_t* knn, int nq, int n_grp, int max_dist, const double* q_bv, const double* q_uv,
+                              const double* grp_wpt, uint32_t* key, double* bv, double* X, double* uv, int32_t* mq, int32_t* mg,
+                              int32_t* count);
+int alva_reloc_pose_launch(alva_ctx* ctx, int cap, const int32_t* counts, const double* bvs, const double* X, const double* uv,
+                           const double* K4, float fx, float fy, uint32_t seed, int max_iter, double* T12, double* info, uint8_t* o1,
+                           double* uv2, double* X2, int32_t* n2, double* pose7, uint8_t* o2, double* summ, double huber, double chi2);
 
 namespace {
 
@@ -103,6 +111,14 @@ struct CudaBackend {
     uint8_t *flag_dev = nullptr, *blur_dev = nullptr, *desc_dev = nullptr;
     int32_t* cnt_dev = nullptr;
     double *quality_dev = nullptr, *dbl_dev = nullptr;   // dbl_dev: [A: 3 cap][B: 3 cap][C: 3 cap][small: 64]
+    // relocalisation: the lost frames' detector quality (quality_dev stays the tracker's), the frozen map's table on the device
+    // (uploaded when its version changes) and the chain's device-only lists (reloc_ws, sized by reloc_ws_cap queries)
+    double* reloc_quality_dev = nullptr;
+    uint8_t *reloc_tab = nullptr, *reloc_ws = nullptr;
+    size_t reloc_tab_bytes = 0;
+    int reloc_ws_cap = 0;
+    unsigned reloc_version = 0;
+    bool reloc_loaded = false;
     bool blur_valid = false;
     // CLAHE (State::claheEnabled_ / claheContrastLimit_ / claheTileSize_, visual_frontend.cpp:16-18, 678-681).  When on, the gray
     // frame goes to raw_dev, its equalised image is level 0: KLT and the detector read the equalised pyramid, ORB describes the
@@ -146,6 +162,8 @@ struct CudaBackend {
         SYS_CUDA(cudaMalloc(&blur_dev, (size_t)W * H));
         const double q0 = 0.001;   // State::extractorMaxQuality_ (state.hpp:59); FeatureExtractor keeps adapting it across resets
         SYS_CUDA(cudaMemcpy(quality_dev, &q0, 8, cudaMemcpyHostToDevice));
+        SYS_CUDA(cudaMalloc(&reloc_quality_dev, 8));
+        SYS_CUDA(cudaMemcpy(reloc_quality_dev, &q0, 8, cudaMemcpyHostToDevice));
         return set_cell(40);   // State(w, h, 40) (system.cpp:15)
     }
 
@@ -193,6 +211,9 @@ struct CudaBackend {
         if (raw_dev) { cudaFree(raw_dev); raw_dev = nullptr; }
         if (clahe_lut) { cudaFree(clahe_lut); clahe_lut = nullptr; clahe_lut_bytes = 0; }
         if (unpx_dev) { cudaFree(unpx_dev); unpx_dev = nullptr; }
+        void** rbufs[] = {(void**)&reloc_quality_dev, (void**)&reloc_tab, (void**)&reloc_ws};
+        for (void** b : rbufs) if (*b) { cudaFree(*b); *b = nullptr; }
+        reloc_tab_bytes = 0; reloc_ws_cap = 0; reloc_loaded = false;
         has_dist = false;
         cap = cap_alloc = 0;
         cell = 40;
@@ -305,14 +326,17 @@ struct CudaBackend {
         return pyramid_launches();
     }
 
-    int detect(const float* cpts, int ncur, std::vector<float>& fresh) {
+    int detect(const float* cpts, int ncur, std::vector<float>& fresh) { return detect_with(cpts, ncur, quality_dev, fresh); }
+    // a lost frame: the whole frame, no current keypoints, the relocalisation's own adaptive quality
+    int detect_lost(std::vector<float>& fresh) { return detect_with(nullptr, 0, reloc_quality_dev, fresh); }
+    int detect_with(const float* cpts, int ncur, double* quality, std::vector<float>& fresh) {
         cudaStream_t st = ctx->stream;
         if (ncur > cap) { alva_set_error("System: %d keypoints exceed the frame capacity %d", ncur, cap); return ALVA_E_CAPACITY; }
         int32_t nc = ncur;
         if (ncur) SYS_CUDA(cudaMemcpyAsync(pts_dev, cpts, (size_t)ncur * 8, cudaMemcpyHostToDevice, st));
         SYS_CUDA(cudaMemcpyAsync(cnt_dev + 1, &nc, 4, cudaMemcpyHostToDevice, st));
         const int32_t roi[4] = {20, 20, w - 40, h - 40};   // CameraCalibration(..., imgBorder 20): roi_rect_ (camera_calibration.cpp:21)
-        if (int e = alva_k_detect_grid(ctx, img[cur][0], w, h, 1, cell, pts_dev, cnt_dev + 1, cap, roi, quality_dev, pri_dev, nullptr, cnt_dev, cap))
+        if (int e = alva_k_detect_grid(ctx, img[cur][0], w, h, 1, cell, pts_dev, cnt_dev + 1, cap, roi, quality, pri_dev, nullptr, cnt_dev, cap))
             return e;
         if (has_dist)   // Frame::computeKeypoint's undistortImagePoint of every new keypoint (frame.cpp:101-109)
             if (int e = alva_undistort_points_launch(ctx, pri_dev, cnt_dev, 1, cap, K4, D4, unpx_dev)) return e;
@@ -482,6 +506,89 @@ struct CudaBackend {
         ok2 = hs[24 + 10] != 0.0 ? 1 : 0;
         memcpy(o1, ho1, n);
         memcpy(o2, ho2, n);
+        return 0;
+    }
+
+    // A lost frame against the frozen map, ONE upload of the queries, ONE download and ONE synchronisation: grouped Hamming 2-NN
+    // -> match rules (gate 51 = 0.2 * 256, mapMaxDescriptorDistance_; ratio 0.8; one query per map point) -> P3P-RANSAC (512
+    // hypotheses, the tracker's seed and 3-px threshold) -> hand-over -> PnP with the tracker's options.  The table is uploaded
+    // once per loss (its version changes when the core rebuilds it).
+    int relocalise(const alva_sys::RelocTable& T, const uint8_t* qdesc, const double* qbv, const double* quv, int nq, const double* K4h,
+                   float fxf, float fyf, alva_sys::RelocResult& R) {
+        cudaStream_t st = ctx->stream;
+        R = alva_sys::RelocResult();
+        const int n_grp = (int)T.mp_id.size(), n_rows = (int)(T.desc.size() / 32);
+        if (nq > cap) { alva_set_error("System: %d queries exceed the frame capacity %d", nq, cap); return ALVA_E_CAPACITY; }
+        if (nq == 0 || n_grp == 0) return 0;
+        const size_t ds_b = al256((size_t)(n_grp + 1) * 4), w_b = al256((size_t)n_grp * 24), d_b = al256((size_t)n_rows * 32),
+                     k_b = al256((size_t)n_grp * 4);
+        if (!reloc_loaded || reloc_version != T.version) {
+            if (ds_b + w_b + d_b + k_b > reloc_tab_bytes) {
+                if (reloc_tab) { SYS_CUDA(cudaStreamSynchronize(st)); cudaFree(reloc_tab); reloc_tab = nullptr; reloc_tab_bytes = 0; }
+                SYS_CUDA(cudaMalloc(&reloc_tab, ds_b + w_b + d_b + k_b));
+                reloc_tab_bytes = ds_b + w_b + d_b + k_b;
+            }
+            SYS_CUDA(cudaMemcpyAsync(reloc_tab, T.desc_start.data(), (size_t)(n_grp + 1) * 4, cudaMemcpyHostToDevice, st));
+            SYS_CUDA(cudaMemcpyAsync(reloc_tab + ds_b, T.wpt.data(), (size_t)n_grp * 24, cudaMemcpyHostToDevice, st));
+            SYS_CUDA(cudaMemcpyAsync(reloc_tab + ds_b + w_b, T.desc.data(), (size_t)n_rows * 32, cudaMemcpyHostToDevice, st));
+            reloc_version = T.version;
+            reloc_loaded = true;
+        }
+        const int32_t* d_start = (const int32_t*)reloc_tab;
+        const double* d_wpt = (const double*)(reloc_tab + ds_b);
+        const uint8_t* d_desc = reloc_tab + ds_b + w_b;
+        uint32_t* d_key = (uint32_t*)(reloc_tab + ds_b + w_b + d_b);
+        if (cap > reloc_ws_cap) {   // device-only lists: knn [4], bv / X [3], uv [2], uv2 [2], X2 [3] per query
+            if (reloc_ws) { SYS_CUDA(cudaStreamSynchronize(st)); cudaFree(reloc_ws); reloc_ws = nullptr; reloc_ws_cap = 0; }
+            SYS_CUDA(cudaMalloc(&reloc_ws, (size_t)cap * 128 + 8 * 256));
+            reloc_ws_cap = cap;
+        }
+        const size_t c = (size_t)cap;
+        int32_t* d_knn = (int32_t*)reloc_ws;
+        double* d_bv = (double*)(reloc_ws + al256(c * 16));
+        double* d_X = d_bv + 3 * c;
+        double* d_uv = d_X + 3 * c;
+        double* d_uv2 = d_uv + 2 * c;
+        double* d_X2 = d_uv2 + 2 * c;
+        stg.reset();
+        uint8_t* hq;
+        double *hb, *hu, *hk, *hs;
+        int32_t *hmq, *hmg;
+        uint8_t *ho1, *ho2;
+        uint8_t* dq = stg.take<uint8_t>((size_t)32 * nq, &hq);
+        double* db = stg.take<double>((size_t)3 * nq, &hb);
+        double* du = stg.take<double>((size_t)2 * nq, &hu);
+        double* dk = stg.take<double>(4, &hk);
+        const size_t up_end = stg.off;
+        double* ds = stg.take<double>(48, &hs);   // [0,12) T12  [12,16) RANSAC info  [16,23) pose7  [24,36) PnP summary  [40] #matches  [41] n2
+        const size_t down_off = (uint8_t*)ds - stg.d;
+        int32_t* dmq = stg.take<int32_t>(nq, &hmq);
+        int32_t* dmg = stg.take<int32_t>(nq, &hmg);
+        uint8_t* do1 = stg.take<uint8_t>(nq, &ho1);
+        uint8_t* do2 = stg.take<uint8_t>(nq, &ho2);
+        const size_t down_end = stg.off;
+        if (!stg.fits(stg.off)) { alva_set_error("System: staging buffer too small for %d queries", nq); return ALVA_E_CAPACITY; }
+        memcpy(hq, qdesc, (size_t)32 * nq); memcpy(hb, qbv, (size_t)24 * nq); memcpy(hu, quv, (size_t)16 * nq); memcpy(hk, K4h, 32);
+        SYS_CUDA(cudaMemcpyAsync(stg.d, stg.h, up_end, cudaMemcpyHostToDevice, st));
+        int32_t* d_cnt = (int32_t*)(ds + 40);
+        int32_t* d_n2 = (int32_t*)(ds + 41);
+        if (int e = alva_k_hamming_knn2_grouped(ctx, dq, nq, d_start, n_grp, d_desc, n_rows, d_knn)) return e;
+        if (int e = alva_reloc_compact_launch(ctx, d_knn, nq, n_grp, 51, db, du, d_wpt, d_key, d_bv, d_X, d_uv, dmq, dmg, d_cnt)) return e;
+        const float chi2 = 5.9915f;   // State::robustCostThreshold_; ceresPnP: Huber width std::sqrt(float)
+        if (int e = alva_reloc_pose_launch(ctx, nq, d_cnt, d_bv, d_X, d_uv, dk, fxf, fyf, 12345u, 512, ds, ds + 12, do1, d_uv2, d_X2, d_n2, ds + 16,
+                                           do2, ds + 24, (double)sqrtf(chi2), (double)chi2))
+            return e;
+        SYS_CUDA(cudaMemcpyAsync(stg.h + down_off, stg.d + down_off, down_end - down_off, cudaMemcpyDeviceToHost, st));
+        SYS_CUDA(cudaStreamSynchronize(st));
+        R.n_match = *(int32_t*)(hs + 40);
+        memcpy(R.T12, hs, 96);
+        R.ok1 = hs[12] != 0.0 ? 1 : 0;
+        memcpy(R.pose7, hs + 16, 56);
+        R.ok2 = hs[24 + 10] != 0.0 ? 1 : 0;
+        R.mq.assign(hmq, hmq + R.n_match);
+        R.mg.assign(hmg, hmg + R.n_match);
+        R.o1.assign(ho1, ho1 + R.n_match);
+        R.o2.assign(ho2, ho2 + R.n_match);
         return 0;
     }
 
@@ -736,6 +843,11 @@ public:
         return n;
     }
     int getPose(double* Twc7) { core_.cur.Twc.to7(Twc7); return 0; }
+    int setRelocalisation(int max_lost_frames) {
+        if (!configured_) { alva_set_error("System: not configured"); return ALVA_E_STATE; }
+        core_.setRelocalisation(max_lost_frames);
+        return 0;
+    }
     // page-lock a caller-owned frame buffer that is reused from call to call (the reference's shim allocates its image buffer once,
     // system.js:63-67): uploads from it then run at the host link's rate instead of through the driver's pageable staging
     int pinBuffer(void* ptr, size_t bytes) {
@@ -821,6 +933,10 @@ extern "C" int alva_system_set_distortion(alva_system* s, double k1, double k2, 
 extern "C" int alva_system_set_preset(alva_system* s, int preset) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
     if (!s) { alva_set_error("alva_system_set_preset: null handle"); return ALVA_E_INVALID; }
     return s->sys.setPreset(preset);
+}
+extern "C" int alva_system_set_relocalisation(alva_system* s, int max_lost_frames) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
+    if (!s || max_lost_frames < 0) { alva_set_error("alva_system_set_relocalisation: bad argument"); return ALVA_E_INVALID; }
+    return s->sys.setRelocalisation(max_lost_frames);
 }
 extern "C" int alva_system_reset(alva_system* s) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1); if (!s) return ALVA_E_INVALID; s->sys.reset(); return 0; }
 extern "C" int alva_system_find_camera_pose(alva_system* s, const uint8_t* rgba, float* pose16) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);

@@ -442,6 +442,11 @@ template <class B> struct BackendHasPoseChain<B, std::void_t<decltype(std::declv
 template <class B, class = void> struct BackendHasUnpx : std::false_type {};
 template <class B> struct BackendHasUnpx<B, std::void_t<decltype(std::declval<B&>().unpx())>> : std::true_type {};
 
+// a Backend may relocalise a lost frame against the map (detect_lost + relocalise); with one that cannot, the relocalisation
+// mode has no effect (the test suite's older CPU backends)
+template <class B, class = void> struct BackendHasReloc : std::false_type {};
+template <class B> struct BackendHasReloc<B, std::void_t<decltype(std::declval<B&>().detect_lost(std::declval<std::vector<float>&>()))>> : std::true_type {};
+
 // ------------------------------------------------------------------------------------------------ flat problems handed to a Backend
 struct BaProblem {   // the layout of alva_k_ba_local
     int nkf = 0, nlm = 0, nobs = 0;
@@ -472,6 +477,25 @@ struct MatchProblem {   // Mapper::matchToMap on flat arrays (the contract of al
     bool has_dist = false;              // lens distortion of the projections (Camera::dist)
     double dist[4] = {0, 0, 0, 0};
 };
+// the map a lost frame is matched against: every map point that is 3-D and has a descriptor, in ascending id order; its
+// keyframe descriptors (MapPoint::kfdesc) in ascending keyframe id order, CSR.  The map is frozen while lost: built once, when
+// the core enters LOST; `version` tells a backend that keeps a device copy when to upload it again.
+struct RelocTable {
+    std::vector<int32_t> mp_id;         // [n]
+    std::vector<double> wpt;            // [n][3]
+    std::vector<int32_t> desc_start;    // [n + 1]
+    std::vector<uint8_t> desc;          // [rows][32]
+    unsigned version = 0;
+    void clear() { mp_id.clear(); wpt.clear(); desc_start.clear(); desc.clear(); version++; }
+};
+// what Backend::relocalise returns: the kept matches (query, table row) in ascending query order; P3P-RANSAC on them (T12, ok1,
+// o1 [n_match]); PnP from the RANSAC pose on its inliers (pose7, ok2, o2 [n_match - #o1], in the inliers' order)
+struct RelocResult {
+    int n_match = 0, ok1 = 0, ok2 = 0;
+    std::vector<int32_t> mq, mg;
+    double T12[12] = {0}, pose7[7] = {0};
+    std::vector<uint8_t> o1, o2;
+};
 
 // ------------------------------------------------------------------------------------------------ the state machine
 // Backend concept (host pointers in, host pointers out; < 0 = ALVA_E_* error):
@@ -488,6 +512,10 @@ struct MatchProblem {   // Mapper::matchToMap on flat arrays (the contract of al
 //   int triangulate(const double* Tlr7, const double* bvl, const double* bvr, int n, double* out)
 //   bool has_ba_local(); int ba_local(BaProblem& io, int32_t* flags)         Optimizer::localBA's numerical body (two solves + flags)
 //   bool has_match_to_map(); int match_to_map(const MatchProblem&, std::vector<int>& kp_match)   Mapper::matchToMap
+//   int detect_lost(std::vector<float>& fresh)             grid detector on the whole current image with its own adaptive quality
+//                                                          (the tracker's is left as it was); unpx() as after detect()
+//   int relocalise(const RelocTable&, const uint8_t* qdesc, const double* qbv, const double* quv, int nq, const double* K4,
+//                  float fx, float fy, RelocResult&)       grouped Hamming 2-NN, match rules, P3P-RANSAC (512) and PnP (relocaliseFrame)
 //   optional: const float* unpx()                          see BackendHasUnpx
 template <class Backend>
 class SystemCore {
@@ -500,7 +528,11 @@ public:
         const double zero[4] = {0, 0, 0, 0};
         cam.setDistortion(zero);
         setPreset(40, 0.95f, true);   // State(w, h, 40), mapKeyframeFilteringRatio_ 0.95, p3pEnabled_ (system.cpp:15-19)
+        reloc_max = 0;
     }
+
+    // relocalisation after a tracking loss (0 = off: the reference's reset on the fourth failed pose); kept by reset()
+    void setRelocalisation(int max_lost_frames) { reloc_max = max_lost_frames; }
 
     // The fields of the reference's preset table (state.hpp:9-17) the state machine reads: State(w, h, cell) and its
     // frameMaxNumKeypoints_ (state.cpp:3-12), the current Frame's grid (Frame(calibration, cell), frame.cpp:9-15), the keyframe
@@ -527,16 +559,28 @@ public:
         n_mp_ids = n_kf_ids = n_kf = 0;
         ready_for_init = reset_requested = false;
         pose_failed = 0;
+        lost = false; lost_frames = 0;
+        reloc_table.clear();
         // VisualFrontend::reset leaves the motion model and p3pReq_ alone (visual_frontend.cpp:718-728); so does this
     }
 
-    // System::processCameraPose: returns 1 tracking / 2 reset / 3 not initialised, or a negative backend error
+    // System::processCameraPose: returns 1 tracking / 2 reset / 3 not initialised / 4 lost (relocalisation on), or a negative
+    // backend error
     int process(const uint8_t* rgba, double timestamp) {
         cur.id++;
         cur.ts = timestamp;
         err = 0;
-        const bool kf = frontend(rgba, timestamp);
-        if (err) return err;
+        bool kf = false;
+        if (lost) {
+            if constexpr (BackendHasReloc<Backend>::value) {
+                const int st = relocaliseFrame(rgba, timestamp, kf);
+                if (st != 1) return st;
+            }
+        } else {
+            kf = frontend(rgba, timestamp);
+            if (err) return err;
+            if (lost) return 4;
+        }
         if (kf) {
             createKeyframe();
             if (err) return err;
@@ -652,6 +696,10 @@ public:
     std::vector<float> parallax_scratch;
 
     // ---- state the facade reads
+    int reloc_max = 0;               // frames a lost track may relocalise for (0: off)
+    bool lost = false;
+    int lost_frames = 0;             // consecutive frames returned as lost
+    RelocTable reloc_table;
     Camera cam;
     Frame cur;
     std::unordered_map<int, std::shared_ptr<Frame>> keyframes;   // MapManager::mapKeyframes_
@@ -665,6 +713,8 @@ public:
     // motion prior, failures of that PnP (p3pReq_ set for the next frame), local BA solves, and solves in which the 21-free-pose
     // limit below held keyframes fixed
     int n_pnp_prior = 0, n_p3p_fallback = 0, n_local_ba = 0, n_free_pose_clamp = 0;
+    // relocalisation: times the track was lost, frames relocalised, and the matches / PnP inliers of the last attempt
+    int n_lost = 0, n_relocalised = 0, reloc_last_matches = 0, reloc_last_inliers = 0;
 
 private:
     Backend& B;
@@ -1181,6 +1231,7 @@ private:
         err = 0;
         if (cur.id == 0) return true;
         Se3 Twc = cur.Twc;
+        const Se3 tracked = cur.Twc;
         motion.apply(Twc, timestamp);
         cur.setTwc(Twc);
         kltTracking();
@@ -1192,12 +1243,114 @@ private:
         }
         const bool ok = computePose();
         if (err) return false;
+        if (!ok && reloc_max > 0 && BackendHasReloc<Backend>::value) { enterLost(tracked); return false; }
         if (!ok) {
             pose_failed++;
             if (pose_failed > 3) { reset_requested = true; return false; }
         }
         motion.update(cur.Twc, timestamp);
         return checkNewKeyframeRequired();
+    }
+
+    // ------------------------------------------------------------------ relocalisation (not in the reference)
+    // the first failed pose after the initialisation: the frame is emptied, the last tracked pose kept, the map frozen and
+    // its descriptor table built for the lost frames that follow
+    void enterLost(const Se3& tracked) {
+        resetFrame();
+        cur.setTwc(tracked);
+        lost = true;
+        lost_frames = 1;
+        n_lost++;
+        RelocTable& t = reloc_table;
+        t.clear();
+        std::vector<int> ids;
+        for (auto& kv : mappoints)
+            if (kv.second.is3d && !kv.second.kfdesc.empty()) ids.push_back(kv.first);
+        std::sort(ids.begin(), ids.end());
+        t.desc_start.push_back(0);
+        for (int id : ids) {
+            const MapPoint& mp = mappoints.at(id);
+            std::vector<int> kfs;
+            for (auto& kv : mp.kfdesc) kfs.push_back(kv.first);
+            std::sort(kfs.begin(), kfs.end());
+            t.mp_id.push_back(id);
+            t.wpt.insert(t.wpt.end(), mp.p, mp.p + 3);
+            for (int k : kfs) { const Desc& d = mp.kfdesc.at(k); t.desc.insert(t.desc.end(), d.b, d.b + 32); }
+            t.desc_start.push_back((int32_t)(t.desc.size() / 32));
+        }
+    }
+
+    // one lost frame: pyramid (KLT's previous level once tracking resumes), grid detector over the whole frame, ORB on the raw
+    // image, then Backend::relocalise against the frozen map.  Returns 1 relocalised (kf: the reference's keyframe decision
+    // for this frame), 4 still lost, 2 gave up (reset, as the reference), or a negative backend error.
+    int relocaliseFrame(const uint8_t* rgba, double timestamp, bool& kf) {
+        kf = false;
+        if ((err = B.pyramid(rgba)) < 0) return err;
+        err = 0;
+        std::vector<float> fresh;
+        if ((err = B.detect_lost(fresh)) < 0) return err;
+        err = 0;
+        const float* un = backendUnpx();
+        std::vector<float> fresh_un;
+        if (un) fresh_un.assign(un, un + fresh.size());
+        const int nn = (int)fresh.size() / 2;
+        std::vector<uint8_t> desc(32 * (size_t)nn + 32), kept(nn + 1);
+        if (nn > 0 && (err = B.describe(fresh.data(), nn, desc.data(), kept.data())) < 0) return err;
+        err = 0;
+        std::vector<Keypoint> qk;                    // the queries: points ORB kept, in detector order
+        std::vector<uint8_t> qdesc;
+        std::vector<double> qbv, quv;
+        for (int i = 0; i < nn; i++) {
+            if (!kept[i]) continue;
+            Keypoint k;
+            cur.compute(fresh[2 * i], fresh[2 * i + 1], k, un ? &fresh_un[2 * (size_t)i] : nullptr);
+            memcpy(k.desc, &desc[32 * (size_t)i], 32);
+            k.has_desc = true;
+            qdesc.insert(qdesc.end(), k.desc, k.desc + 32);
+            qbv.insert(qbv.end(), k.bv, k.bv + 3);
+            quv.push_back(k.ux); quv.push_back(k.uy);
+            qk.push_back(k);
+        }
+        const double K4[4] = {(double)(float)cam.fx, (double)(float)cam.fy, (double)(float)cam.cx, (double)(float)cam.cy};
+        RelocResult R;
+        if ((err = B.relocalise(reloc_table, qdesc.data(), qbv.data(), quv.data(), (int)qk.size(), K4, (float)cam.fx, (float)cam.fy, R)) < 0)
+            return err;
+        err = 0;
+        // the decisions: >= 30 matches, a RANSAC model, PnP with >= 30 inliers that flags at most half of its input
+        const double tt[3] = {R.T12[3], R.T12[7], R.T12[11]};
+        bool ok = R.n_match >= 30 && R.ok1 && finite3(tt) && R.ok2 && finite3(R.pose7);
+        std::vector<int> surv;                       // RANSAC inliers: indices into the matches
+        for (int i = 0; ok && i < R.n_match; i++) if (!R.o1[i]) surv.push_back(i);
+        int nout2 = 0;
+        for (size_t i = 0; ok && i < surv.size(); i++) nout2 += R.o2[i] != 0;
+        const int n2 = (int)surv.size();
+        ok = ok && n2 - nout2 >= 30 && nout2 <= 0.5 * n2;
+        reloc_last_matches = R.n_match;
+        reloc_last_inliers = ok ? n2 - nout2 : 0;
+        if (!ok) {
+            if (++lost_frames > reloc_max) { reset(); return 2; }
+            return 4;
+        }
+        // the PnP inliers become the frame's keypoints, observing their map points
+        for (int s2 = 0; s2 < n2; s2++) {
+            if (R.o2[s2]) continue;
+            const int m = surv[s2];
+            Keypoint k = qk[R.mq[m]];
+            k.id = reloc_table.mp_id[R.mg[m]];
+            k.is3d = true;
+            auto mp = mappoints.find(k.id);
+            if (mp == mappoints.end()) continue;
+            mp->second.observed = true;
+            cur.add(k);
+        }
+        cur.setTwc(Se3::from7(R.pose7));
+        motion.reset();                              // the gap makes the last velocity meaningless
+        motion.update(cur.Twc, timestamp);
+        lost = false;
+        lost_frames = 0;
+        n_relocalised++;
+        kf = checkNewKeyframeRequired();
+        return 1;
     }
 
     void kltTracking() {   // kltTrackingFromMotionPrior (kltUsePrior_ = true)

@@ -69,6 +69,8 @@ _OPTIONAL = {
     "alva_k_undistort_points": [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp],
     "alva_k_project_points": [_vp, _vp, _i32, _vp, _vp, _vp],
     "alva_k_p3p_lmeds": [_vp, _i32, _i32, _vp, _vp, _vp, _i32, C.c_float, C.c_float, C.c_float, C.c_uint32, _vp, _vp, _vp],
+    "alva_k_p3p_ransac": [_vp, _i32, _i32, _vp, _vp, _vp, _i32, C.c_float, C.c_float, C.c_float, C.c_uint32, _vp, _vp, _vp],
+    "alva_k_hamming_knn2_grouped": [_vp, _vp, _i32, _vp, _i32, _vp, _i32, _vp],
     "alva_k_pnp": [_vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, C.c_double, C.c_double, _i32, _i32, _i32, _vp, _vp],
     "alva_k_essential_5pt": [_vp, _i32, _i32, _vp, _vp, _vp, _i32, C.c_float, _i32, C.c_float, C.c_float, C.c_uint32, _vp, _vp, _vp],
     "alva_k_triangulate": [_vp, _vp, _vp, _vp, _i32, _vp],
@@ -248,6 +250,16 @@ class Context:
         """MultiViewGeometry::p3pRansac (Kneip P3P + LMedS), batched -- see alva_k_p3p_lmeds."""
         self._chk(self.L.alva_k_p3p_lmeds(self.h, nprob, cap, _ptr(bvs), _ptr(wpts), _ptr(counts), max_iter, err_px, fx, fy,
                                           seed, _ptr(Twc_out), _ptr(outlier), _ptr(info)))
+
+    def p3p_ransac(self, nprob, cap, bvs, wpts, counts, Twc_out, outlier, info=None, max_iter=512, err_px=3.0, fx=1.0, fy=1.0,
+                   seed=12345):
+        """P3P-RANSAC (the hypotheses of p3p_lmeds scored by inlier count), batched -- see alva_k_p3p_ransac."""
+        self._chk(self.L.alva_k_p3p_ransac(self.h, nprob, cap, _ptr(bvs), _ptr(wpts), _ptr(counts), max_iter, err_px, fx, fy,
+                                           seed, _ptr(Twc_out), _ptr(outlier), _ptr(info)))
+
+    def hamming_knn2_grouped(self, q, nq, desc_start, n_grp, desc, n_rows, out):
+        """Hamming 2-NN over CSR groups of descriptors (min over a group's rows) -- see alva_k_hamming_knn2_grouped."""
+        self._chk(self.L.alva_k_hamming_knn2_grouped(self.h, _ptr(q), nq, _ptr(desc_start), n_grp, _ptr(desc), n_rows, _ptr(out)))
 
     def essential_5pt(self, nprob, cap, bv1, bv2, counts, Rt_out, outlier, info=None, max_iter=100, err_px=3.0, optimize=True,
                       fx=1.0, fy=1.0, seed=12345):

@@ -20,6 +20,7 @@ def _bind():
     L.alva_system_set_clahe.argtypes = [_vp, _i32, _f64, _i32]
     L.alva_system_set_distortion.argtypes = [_vp] + [_f64] * 4
     L.alva_system_set_preset.argtypes = [_vp, _i32]
+    L.alva_system_set_relocalisation.argtypes = [_vp, _i32]
     L.alva_system_num_matched.argtypes = [_vp]
     L.alva_system_configure.argtypes = [_vp, _i32, _i32] + [_f64] * 8
     L.alva_system_find_camera_pose.argtypes = [_vp, _vp, _vp]
@@ -39,7 +40,10 @@ def _bind():
 
 
 class System:
-    """One camera stream.  status codes as the reference: 1 tracking, 2 the tracker was reset during the call, 3 not initialised."""
+    """One camera stream.  Status codes of find_camera_pose: 1 tracking, 2 the tracker was reset during the call, 3 not
+    initialised (the reference's), and 4 lost -- tracking lost, map kept, relocalising (only with set_relocalisation on)."""
+
+    TRACKING, RESET, NOT_INITIALISED, LOST = 1, 2, 3, 4
 
     def __init__(self, width, height, fx, fy, cx, cy, k1=0.0, k2=0.0, p1=0.0, p2=0.0, device=0):
         self.L = _bind()
@@ -153,3 +157,15 @@ class System:
         rc = self.L.alva_system_set_distortion(self.h, float(k1), float(k2), float(p1), float(p2))
         if rc != 0:
             raise AlvaError(f"alva_system_set_distortion -> {rc}: {self.L.alva_last_error().decode()}")
+
+    def set_relocalisation(self, max_lost_frames):
+        """Relocalise against the kept map after a tracking loss instead of discarding it.  0 (the default) is the reference's
+        behaviour: a failed pose empties the frame and the fourth failure since the last reset resets the map (status 2).
+        With n > 0 a failed pose returns status 4 (LOST) with the last tracked pose; the map, keyframes and motion model are
+        frozen and every following frame is matched against the whole map (P3P-RANSAC + PnP).  Tracking resumes with status 1
+        when that succeeds; after n lost frames in a row the map is reset as the reference would (status 2).  Status codes:
+        1 tracking, 2 reset during the call, 3 not initialised, 4 lost.  A new System starts with it off; reset(),
+        set_preset(), set_distortion() and set_clahe() keep it."""
+        rc = self.L.alva_system_set_relocalisation(self.h, int(max_lost_frames))
+        if rc != 0:
+            raise AlvaError(f"alva_system_set_relocalisation -> {rc}: {self.L.alva_last_error().decode()}")

@@ -152,6 +152,15 @@ int alva_k_hamming_knn2(alva_ctx*, const uint8_t* q, int nq, const uint8_t* t, i
 int alva_k_hamming_knn2_batch(alva_ctx*, const uint8_t* q, const int32_t* counts, int nbatch, int qcap,
                               const uint8_t* t, int nt, int32_t* out);
 
+/* Hamming 2-NN over GROUPS of descriptors (System's relocalisation: a map point is a group of the descriptors its keyframes
+ * gave it).  q [nq][32]; the table is CSR: desc_start [n_grp + 1] (ascending, desc_start[0] = 0, desc_start[n_grp] = n_rows)
+ * row offsets into desc [n_rows][32].  A group's distance to a query is the minimum over its rows; groups without rows are never
+ * candidates.  out [nq][4] = {grp0, d0, grp1, d1} (int32, 16-byte aligned): the nearest and second-nearest groups, ties to the
+ * lower group index, -1 / -1 where there are fewer than 1 / 2 candidates.  DEVICE pointers (q, desc 16-byte aligned);
+ * nq <= 65535. */
+int alva_k_hamming_knn2_grouped(alva_ctx*, const uint8_t* q, int nq, const int32_t* desc_start, int n_grp, const uint8_t* desc,
+                                int n_rows, int32_t* out);
+
 /* The reference's keyframe corner detector, FeatureExtractor::detectFeaturePoints(image, cell, currKeypoints, roi)
  * (src/slam/src/feature_extractor.cpp:11-158; caller MapManager::extractKeypoints, map_manager.cpp:193-222), batched over frames:
  * per empty grid cell, GaussianBlur 3x3 -> cornerMinEigenVal(block 3, Sobel 3) -> best and second-best maximum under a shared
@@ -208,6 +217,16 @@ int alva_k_klt_fb(alva_ctx*, const uint8_t* const* prev_img, const int16_t* cons
 int alva_k_p3p_lmeds(alva_ctx*, int nprob, int cap, const double* bvs, const double* wpts, const int32_t* counts,
                      int max_iter, float err_px, float fx, float fy, uint32_t seed, double* Twc_out, uint8_t* outlier,
                      double* info);
+
+/* P3P-RANSAC with the arguments and outputs of alva_k_p3p_lmeds: the same sampler and Kneip hypotheses (the same seed draws the
+ * same hypotheses), each scored by its number of inliers (bearing distance <= 1 - cos(atan(err_px / focal))); the first
+ * hypothesis with the strictly largest count is the model (none without inliers).  Survives outlier shares where LMedS
+ * breaks down (> 50 %): System's relocalisation, whose matches carry no pose prior.  cap <= 8192, max_iter <= 1024.
+ * info (optional) [nprob][4] = {success (>= 5 inliers and R orthogonal), #inliers, index of the selected hypothesis (-1: none),
+ * #draws}. */
+int alva_k_p3p_ransac(alva_ctx*, int nprob, int cap, const double* bvs, const double* wpts, const int32_t* counts,
+                      int max_iter, float err_px, float fx, float fy, uint32_t seed, double* Twc_out, uint8_t* outlier,
+                      double* info);
 
 /* Per-frame pose, step 2: MultiViewGeometry::ceresPnP (src/slam/src/multi_view_geometry.cpp:129-223; functor
  * DirectSE3::ReprojectionErrorSE3, ceres_parametrization.cpp:96-155): Levenberg-Marquardt on the 6-dof pose with
@@ -415,7 +434,7 @@ void* alva_pipeline_buffer(alva_pipeline*, int which);
  * (reference src/slam/src/system.hpp:28-38; JS caller src/system.js:58-237).  Host pointers, caller-owned buffers:
  * rgba = W*H*4 bytes (read only), pose16 = 16 floats (R rows in [0..2],[4..6],[8..10], t in [12..14], [15] = 1;
  * src/slam/src/utils.cpp:3-27).  findCameraPose returns 1 tracking / 2 tracker was reset / 3 not initialised
- * (system.cpp:163-174) or a negative ALVA_E_* code. */
+ * (system.cpp:163-174), ALVA_STATUS_LOST (4, only with alva_system_set_relocalisation on) or a negative ALVA_E_* code. */
 alva_system* alva_system_create(int device);
 void alva_system_destroy(alva_system*);
 int  alva_system_configure(alva_system*, int w, int h, double fx, double fy, double cx, double cy,
@@ -449,6 +468,17 @@ int  alva_system_set_distortion(alva_system*, double k1, double k2, double p1, d
 #define ALVA_PRESET_AVERAGE  2
 #define ALVA_PRESET_ACCURATE 3
 int  alva_system_set_preset(alva_system*, int preset);
+/* Relocalisation instead of a reset after a tracking loss.  max_lost_frames = 0 (the default): the reference's behaviour -- a
+ * failed pose empties the frame and the fourth failure since the last reset discards the map (status 2).  n > 0: the first
+ * failed pose after the initialisation freezes the map, the keyframes and the motion model and returns ALVA_STATUS_LOST; every
+ * following frame is matched against the whole map (grid detector + ORB, Hamming 2-NN over each map point's keyframe
+ * descriptors, distance <= 51 and ratio 0.8, P3P-RANSAC with 512 hypotheses, PnP) and tracking resumes with status 1 once >= 30
+ * PnP inliers agree.  After n lost frames in a row the map is discarded as the reference would (status 2).  While lost, pose16
+ * holds the last tracked pose and the frame has no keypoints.  configure turns it off; reset, set_preset, set_distortion and
+ * set_clahe keep the setting (those that reset the map also end the lost state).  ALVA_E_STATE before configure;
+ * ALVA_E_INVALID for a null handle or a negative value. */
+#define ALVA_STATUS_LOST 4
+int  alva_system_set_relocalisation(alva_system*, int max_lost_frames);
 int  alva_system_find_camera_pose(alva_system*, const uint8_t* rgba, float* pose16);
 /* the same with the frame's time stamp (milliseconds) supplied by the caller instead of read from the system clock
  * (system.cpp:114): deterministic replays, and hosts that deliver frames faster than real time (two frames inside one

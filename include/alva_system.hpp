@@ -31,6 +31,9 @@ public:
     void reset() { alva_system_reset(h_); }
     // not in the reference's class: its FAST / AVERAGE / ACCURATE presets (ALVA_PRESET_*, alva_b200.h); 0 or an ALVA_E_* code
     int setPreset(int preset) { return alva_system_set_preset(h_, preset); }
+    // not in the reference's class: relocalise for up to maxLostFrames frames after a tracking loss instead of resetting
+    // (findCameraPose then returns ALVA_STATUS_LOST while lost; 0 = the reference's reset); 0 or an ALVA_E_* code
+    int setRelocalisation(int maxLostFrames) { return alva_system_set_relocalisation(h_, maxLostFrames); }
 
     // ---- the reference's wasm32 signatures
     int findCameraPose(int imageRGBADataPtr, int posePtr) { return findCameraPose(ptr<const uint8_t>(imageRGBADataPtr), ptr<float>(posePtr)); }
