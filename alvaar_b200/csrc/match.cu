@@ -5,7 +5,8 @@
 //   Mapper::matchToMap                     src/slam/src/mapper.cpp:354-587   (caller matchingToLocalMap :293-352)
 //   MapPoint::computeMinDescDist           src/slam/src/map_point.cpp:204-222  (cv::norm(NORM_HAMMING), all pairs)
 //   Frame::getSurroundingKeypoints         src/slam/src/frame.cpp:313-341
-//   CameraCalibration::projectCamToImageDist  src/slam/src/camera_calibration.cpp:34-55  (with distortion: camera_model.h)
+//   CameraCalibration::projectCamToImageDist  src/slam/src/camera_calibration.cpp:34-55  (with distortion: camera_model.h,
+//                                             radial-tangential or equidistant fisheye)
 //
 // How: the reference walks hash maps (map point -> shared_ptr -> per-keyframe descriptor map -> cv::Mat) once per candidate.
 // Here the map lives in flat SoA arenas in HBM (world points, CSR observation lists, CSR descriptor lists) and one warp
@@ -51,7 +52,7 @@ struct MatchParams {
     int32_t* kp_match;
     float* kp_dist;
     int32_t* n_match;
-    double dist[4];   // k1 k2 p1 p2 of the DIST instantiation
+    double dist[4];   // k1 k2 p1 p2 (LENS_RADTAN) or k1 k2 k3 k4 (LENS_FISHEYE)
 };
 
 __device__ __forceinline__ void quat_R(const double* q, double* R) {
@@ -77,12 +78,16 @@ __device__ __forceinline__ void project(const MatchParams& P, const double* c, f
     px[0] = (float)(x * P.fx + P.cx);
     px[1] = (float)(y * P.fy + P.cy);
 }
-// DIST = false: the zero-distortion projection above; true: the radial-tangential model (camera_model.h)
-template <bool DIST>
+// LENS_NONE: the zero-distortion projection above; LENS_RADTAN / LENS_FISHEYE: the lens models of camera_model.h
+enum { LENS_NONE = 0, LENS_RADTAN = 1, LENS_FISHEYE = 2 };
+template <int LENS>
 __device__ __forceinline__ void project_cam(const MatchParams& P, const double* c, float* px) {
-    if constexpr (DIST) {
+    if constexpr (LENS == LENS_RADTAN) {
         const double K4[4] = {P.fx, P.fy, P.cx, P.cy};
         alva_cam::project_dist(K4, P.dist, c, px);
+    } else if constexpr (LENS == LENS_FISHEYE) {
+        const double K4[4] = {P.fx, P.fy, P.cx, P.cy};
+        alva_cam::project_dist_fisheye(K4, P.dist, c, px);
     } else {
         project(P, c, px);
     }
@@ -130,7 +135,7 @@ __global__ void __launch_bounds__(1024) match_prepare_kernel(const MatchParams P
     }
 }
 
-template <bool DIST>
+template <int LENS>
 __global__ void __launch_bounds__(128) match_local_kernel(const MatchParams P) {
     const int lane = threadIdx.x & 31;
     const int li = (int)((blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5);
@@ -147,7 +152,7 @@ __global__ void __launch_bounds__(128) match_local_kernel(const MatchParams P) {
     const float view_angle = (float)(campt[2] / sqrt(campt[0] * campt[0] + campt[1] * campt[1] + campt[2] * campt[2]));
     if (fabs((double)view_angle) < (double)P.view_th) return;                   // :432
     float proj[2];
-    project_cam<DIST>(P, campt, proj);
+    project_cam<LENS>(P, campt, proj);
     if (!(proj[0] >= 0 && proj[1] >= 0 && (double)proj[0] < (double)P.w && (double)proj[1] < (double)P.h)) return;
     // keyframes observing this map point, as a bit mask over keyframe indices (n_kf <= 64)
     const int o0 = P.obs_start[m], no = P.obs_start[m + 1] - o0;
@@ -189,7 +194,7 @@ __global__ void __launch_bounds__(128) match_local_kernel(const MatchParams P) {
                         double cc[3];
                         float pp[2];
                         world_to_cam(P.kf_Twc + 7 * P.obs_kf[ko0 + a0 + lane], wpt, cc);
-                        project_cam<DIST>(P, cc, pp);
+                        project_cam<LENS>(P, cc, pp);
                         const float ex = P.obs_px[2 * (ko0 + a0 + lane)] - pp[0], ey = P.obs_px[2 * (ko0 + a0 + lane) + 1] - pp[1];
                         dist = sqrt((double)ex * (double)ex + (double)ey * (double)ey);
                     }
@@ -236,14 +241,13 @@ __global__ void match_finalize_kernel(const MatchParams P) {
     atomicAdd(P.n_match, 1);
 }
 
-}  // namespace
-
-extern "C" int alva_k_match_to_map_dist(alva_ctx* ctx, int w, int h, int cell, double fx, double fy, double cx, double cy,
-                                        const double* Twc_cur, int n_kp, const int32_t* kp_mp, const float* kp_px, int nkp3d, int n_kf,
-                                        const double* kf_Twc, int n_mp, const double* mp_wpt, const uint8_t* mp_is3d,
-                                        const int32_t* obs_start, const int32_t* obs_kf, const float* obs_px, const int32_t* desc_start,
-                                        const uint8_t* desc, int n_local, const int32_t* local_mp, float max_proj_err, float dist_ratio,
-                                        int32_t* kp_match, float* kp_dist, int32_t* n_match, const double* dist4) { AlvaDeviceGuard guard__(ctx);
+// lens: LENS_NONE (coef4 unused), LENS_RADTAN or LENS_FISHEYE with its four coefficients (checked by the caller)
+int match_to_map_launch(alva_ctx* ctx, int w, int h, int cell, double fx, double fy, double cx, double cy, const double* Twc_cur,
+                        int n_kp, const int32_t* kp_mp, const float* kp_px, int nkp3d, int n_kf, const double* kf_Twc, int n_mp,
+                        const double* mp_wpt, const uint8_t* mp_is3d, const int32_t* obs_start, const int32_t* obs_kf,
+                        const float* obs_px, const int32_t* desc_start, const uint8_t* desc, int n_local, const int32_t* local_mp,
+                        float max_proj_err, float dist_ratio, int32_t* kp_match, float* kp_dist, int32_t* n_match, int lens,
+                        const double* coef4) {
     if (!ctx || !Twc_cur || !kp_mp || !kp_px || !kf_Twc || !mp_wpt || !mp_is3d || !obs_start || !obs_kf || !obs_px || !desc_start ||
         !desc || !local_mp || !kp_match || !n_match || n_kp < 1 || n_mp < 1 || n_local < 1 || cell < 1) {
         alva_set_error("alva_k_match_to_map: bad argument");
@@ -251,14 +255,8 @@ extern "C" int alva_k_match_to_map_dist(alva_ctx* ctx, int w, int h, int cell, d
     }
     if (n_kf > 64) { alva_set_error("alva_k_match_to_map: at most 64 keyframes (the reference's window is 30), got %d", n_kf); return ALVA_E_INVALID; }
     if (((uintptr_t)desc & 15) != 0) { alva_set_error("alva_k_match_to_map: desc must be 16-byte aligned"); return ALVA_E_INVALID; }
-    bool dist = false;
-    if (dist4)
-        for (int i = 0; i < 4; i++) {
-            if (!isfinite(dist4[i])) { alva_set_error("alva_k_match_to_map_dist: non-finite distortion coefficient"); return ALVA_E_INVALID; }
-            dist = dist || dist4[i] != 0.0;
-        }
     MatchParams P{};
-    if (dist) for (int i = 0; i < 4; i++) P.dist[i] = dist4[i];
+    if (lens != LENS_NONE) for (int i = 0; i < 4; i++) P.dist[i] = coef4[i];
     P.w = w; P.h = h; P.cell = cell;
     P.ncw = (int)ceilf((float)w / (float)cell); P.nch = (int)ceilf((float)h / (float)cell);   // frame.cpp:14-15
     P.fx = fx; P.fy = fy; P.cx = cx; P.cy = cy;
@@ -281,12 +279,46 @@ extern "C" int alva_k_match_to_map_dist(alva_ctx* ctx, int w, int h, int cell, d
     P.kp_match = kp_match; P.kp_dist = kp_dist; P.n_match = n_match;
     match_prepare_kernel<<<1, 1024, 0, ctx->stream>>>(P);
     ALVA_LAUNCH_CHECK(ctx);
-    if (dist) match_local_kernel<true><<<(n_local * 32 + 127) / 128, 128, 0, ctx->stream>>>(P);
-    else match_local_kernel<false><<<(n_local * 32 + 127) / 128, 128, 0, ctx->stream>>>(P);
+    if (lens == LENS_RADTAN) match_local_kernel<LENS_RADTAN><<<(n_local * 32 + 127) / 128, 128, 0, ctx->stream>>>(P);
+    else if (lens == LENS_FISHEYE) match_local_kernel<LENS_FISHEYE><<<(n_local * 32 + 127) / 128, 128, 0, ctx->stream>>>(P);
+    else match_local_kernel<LENS_NONE><<<(n_local * 32 + 127) / 128, 128, 0, ctx->stream>>>(P);
     ALVA_LAUNCH_CHECK(ctx);
     match_finalize_kernel<<<(n_kp + 255) / 256, 256, 0, ctx->stream>>>(P);
     ALVA_LAUNCH_CHECK(ctx);
     return 0;
+}
+
+}  // namespace
+
+extern "C" int alva_k_match_to_map_dist(alva_ctx* ctx, int w, int h, int cell, double fx, double fy, double cx, double cy,
+                                        const double* Twc_cur, int n_kp, const int32_t* kp_mp, const float* kp_px, int nkp3d, int n_kf,
+                                        const double* kf_Twc, int n_mp, const double* mp_wpt, const uint8_t* mp_is3d,
+                                        const int32_t* obs_start, const int32_t* obs_kf, const float* obs_px, const int32_t* desc_start,
+                                        const uint8_t* desc, int n_local, const int32_t* local_mp, float max_proj_err, float dist_ratio,
+                                        int32_t* kp_match, float* kp_dist, int32_t* n_match, const double* dist4) { AlvaDeviceGuard guard__(ctx);
+    bool dist = false;
+    if (dist4)
+        for (int i = 0; i < 4; i++) {
+            if (!isfinite(dist4[i])) { alva_set_error("alva_k_match_to_map_dist: non-finite distortion coefficient"); return ALVA_E_INVALID; }
+            dist = dist || dist4[i] != 0.0;
+        }
+    return match_to_map_launch(ctx, w, h, cell, fx, fy, cx, cy, Twc_cur, n_kp, kp_mp, kp_px, nkp3d, n_kf, kf_Twc, n_mp, mp_wpt, mp_is3d,
+                               obs_start, obs_kf, obs_px, desc_start, desc, n_local, local_mp, max_proj_err, dist_ratio, kp_match, kp_dist,
+                               n_match, dist ? LENS_RADTAN : LENS_NONE, dist4);
+}
+
+extern "C" int alva_k_match_to_map_fisheye(alva_ctx* ctx, int w, int h, int cell, double fx, double fy, double cx, double cy,
+                                           const double* Twc_cur, int n_kp, const int32_t* kp_mp, const float* kp_px, int nkp3d, int n_kf,
+                                           const double* kf_Twc, int n_mp, const double* mp_wpt, const uint8_t* mp_is3d,
+                                           const int32_t* obs_start, const int32_t* obs_kf, const float* obs_px, const int32_t* desc_start,
+                                           const uint8_t* desc, int n_local, const int32_t* local_mp, float max_proj_err, float dist_ratio,
+                                           int32_t* kp_match, float* kp_dist, int32_t* n_match, const double* fisheye4) { AlvaDeviceGuard guard__(ctx);
+    if (!fisheye4) { alva_set_error("alva_k_match_to_map_fisheye: fisheye4 is required (zeros are a valid lens)"); return ALVA_E_INVALID; }
+    for (int i = 0; i < 4; i++)
+        if (!isfinite(fisheye4[i])) { alva_set_error("alva_k_match_to_map_fisheye: non-finite coefficient"); return ALVA_E_INVALID; }
+    return match_to_map_launch(ctx, w, h, cell, fx, fy, cx, cy, Twc_cur, n_kp, kp_mp, kp_px, nkp3d, n_kf, kf_Twc, n_mp, mp_wpt, mp_is3d,
+                               obs_start, obs_kf, obs_px, desc_start, desc, n_local, local_mp, max_proj_err, dist_ratio, kp_match, kp_dist,
+                               n_match, LENS_FISHEYE, fisheye4);
 }
 
 extern "C" int alva_k_match_to_map(alva_ctx* ctx, int w, int h, int cell, double fx, double fy, double cx, double cy,

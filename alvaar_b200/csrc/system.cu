@@ -25,8 +25,9 @@
 //                (not in the reference: alva_system_set_relocalisation)
 // There is no CPU fallback: configure() fails without an sm_90 (H100) device.  Lens distortion: the JS shim always passes zeros
 // (system.js:84-141) and configure() rejects non-zero coefficients; setDistortion() (alva_system_set_distortion) sets them on a
-// configured System.  With distortion on, klt and detect undistort the points they return with alva_k_undistort_points on the
-// device, in the same download (camera.cu, camera_model.h).
+// configured System, and setFisheye() (alva_system_set_fisheye) selects OpenCV's equidistant fisheye model instead.  With a
+// lens on, klt and detect undistort the points they return with alva_k_undistort_points (or its fisheye twin) on the device, in
+// the same download (camera.cu, camera_model.h).
 #include "alva_common.cuh"
 #include "../../include/alva_b200.h"
 #include "system_core.h"
@@ -41,6 +42,8 @@ int alva_clahe_launch(alva_ctx* ctx, const uint8_t* src, uint8_t* dst, int w, in
                       int tiles_y, uint8_t* lut);
 int alva_undistort_points_launch(alva_ctx* ctx, const float* px, const int32_t* counts, int nframes, int cap, const double* K4,
                                  const double* D4, float* unpx);
+int alva_undistort_points_fisheye_launch(alva_ctx* ctx, const float* px, const int32_t* counts, int nframes, int cap, const double* K4,
+                                         const double* D4, float* unpx);
 int alva_pose_chain_launch(alva_ctx* ctx, int n, int cap, const double* bvs, const double* X, const double* uv, const double* K4,
                            float fx, float fy, uint32_t seed, double* T12, double* info, uint8_t* o1, double* uv2, double* X2,
                            int32_t* n2, double* pose7, uint8_t* o2, double* summ, double huber, double chi2);
@@ -131,8 +134,8 @@ struct CudaBackend {
     size_t clahe_lut_bytes = 0;
     cudaGraphExec_t clahe_graph[2] = {nullptr, nullptr};
     // lens distortion (CameraCalibration::D_): when on, klt() and detect() also return the undistorted positions of their points
-    // (unpx()); with it off nothing here is allocated or launched
-    bool has_dist = false;
+    // (unpx()); with it off nothing here is allocated or launched.  fisheye: through the equidistant fisheye model.
+    bool has_dist = false, fisheye = false;
     double K4[4] = {0, 0, 0, 0}, D4[4] = {0, 0, 0, 0};
     float* unpx_dev = nullptr;
     std::vector<float> unpx_host;
@@ -214,7 +217,7 @@ struct CudaBackend {
         void** rbufs[] = {(void**)&reloc_quality_dev, (void**)&reloc_tab, (void**)&reloc_ws};
         for (void** b : rbufs) if (*b) { cudaFree(*b); *b = nullptr; }
         reloc_tab_bytes = 0; reloc_ws_cap = 0; reloc_loaded = false;
-        has_dist = false;
+        has_dist = fisheye = false;
         cap = cap_alloc = 0;
         cell = 40;
         clahe = false;
@@ -247,10 +250,23 @@ struct CudaBackend {
 
     int set_distortion(const double* d) {
         has_dist = d[0] != 0.0 || d[1] != 0.0 || d[2] != 0.0 || d[3] != 0.0;
+        fisheye = false;
         for (int i = 0; i < 4; i++) D4[i] = d[i];
         K4[0] = fx; K4[1] = fy; K4[2] = cx; K4[3] = cy;
         if (has_dist && !unpx_dev) SYS_CUDA(cudaMalloc(&unpx_dev, (size_t)cap_alloc * 8));
         return 0;
+    }
+    int set_fisheye(bool on, const double* k) {
+        has_dist = fisheye = on;
+        for (int i = 0; i < 4; i++) D4[i] = on ? k[i] : 0.0;
+        K4[0] = fx; K4[1] = fy; K4[2] = cx; K4[3] = cy;
+        if (has_dist && !unpx_dev) SYS_CUDA(cudaMalloc(&unpx_dev, (size_t)cap_alloc * 8));
+        return 0;
+    }
+    // Frame::computeKeypoint's undistortImagePoint of the given points, through the lens model that is on
+    int undistort_launch(const float* px, const int32_t* counts, int n, float* unpx) {
+        return fisheye ? alva_undistort_points_fisheye_launch(ctx, px, counts, 1, n, K4, D4, unpx)
+                       : alva_undistort_points_launch(ctx, px, counts, 1, n, K4, D4, unpx);
     }
     const float* unpx() const { return has_dist ? unpx_host.data() : nullptr; }
 
@@ -339,7 +355,7 @@ struct CudaBackend {
         if (int e = alva_k_detect_grid(ctx, img[cur][0], w, h, 1, cell, pts_dev, cnt_dev + 1, cap, roi, quality, pri_dev, nullptr, cnt_dev, cap))
             return e;
         if (has_dist)   // Frame::computeKeypoint's undistortImagePoint of every new keypoint (frame.cpp:101-109)
-            if (int e = alva_undistort_points_launch(ctx, pri_dev, cnt_dev, 1, cap, K4, D4, unpx_dev)) return e;
+            if (int e = undistort_launch(pri_dev, cnt_dev, cap, unpx_dev)) return e;
         int32_t n = 0;
         SYS_CUDA(cudaMemcpyAsync(&n, cnt_dev, 4, cudaMemcpyDeviceToHost, st));
         SYS_CUDA(cudaStreamSynchronize(st));
@@ -391,7 +407,7 @@ struct CudaBackend {
         if (int e = alva_k_klt_fb(ctx, img[prev], der[prev], img[cur], der[cur], w, h, 1, nlev - 1, levels, 9, 30.0f, 0.5f, dp, dq, nullptr, n, dg))
             return e;
         if (has_dist)   // Frame::computeKeypoint's undistortImagePoint of every tracked keypoint (frame.cpp:101-109)
-            if (int e = alva_undistort_points_launch(ctx, dq, nullptr, 1, n, K4, D4, du)) return e;
+            if (int e = undistort_launch(dq, nullptr, n, du)) return e;
         SYS_CUDA(cudaMemcpyAsync(stg.h + q_off, stg.d + q_off, stg.off - q_off, cudaMemcpyDeviceToHost, st));
         SYS_CUDA(cudaStreamSynchronize(st));
         memcpy(priors, hq, (size_t)n * 8);
@@ -671,9 +687,14 @@ struct CudaBackend {
         int32_t* lm = arena_put(m.local_mp.data(), n_local);
         int32_t* out = arena_take<int32_t>(n_kp);
         int32_t* nm = arena_take<int32_t>(4);
-        if (int e = alva_k_match_to_map_dist(ctx, w, h, cell, fx, fy, cx, cy, Tc, (int)n_kp, kpmp, kppx, m.nkp3d, (int)(n_kf ? n_kf : 1), kfT, (int)n_mp,
-                                             wpt, is3, os, ok, op, ds, dd, (int)n_local, lm, 2.0f, 0.2f, out, nullptr, nm, m.has_dist ? m.dist : nullptr))
+        if (m.fisheye) {
+            if (int e = alva_k_match_to_map_fisheye(ctx, w, h, cell, fx, fy, cx, cy, Tc, (int)n_kp, kpmp, kppx, m.nkp3d, (int)(n_kf ? n_kf : 1), kfT,
+                                                    (int)n_mp, wpt, is3, os, ok, op, ds, dd, (int)n_local, lm, 2.0f, 0.2f, out, nullptr, nm, m.dist))
+                return e;
+        } else if (int e = alva_k_match_to_map_dist(ctx, w, h, cell, fx, fy, cx, cy, Tc, (int)n_kp, kpmp, kppx, m.nkp3d, (int)(n_kf ? n_kf : 1), kfT, (int)n_mp,
+                                                    wpt, is3, os, ok, op, ds, dd, (int)n_local, lm, 2.0f, 0.2f, out, nullptr, nm, m.has_dist ? m.dist : nullptr)) {
             return e;
+        }
         std::vector<int32_t> host(n_kp);
         SYS_CUDA(cudaMemcpyAsync(host.data(), out, n_kp * 4, cudaMemcpyDeviceToHost, st));
         SYS_CUDA(cudaStreamSynchronize(st));
@@ -735,6 +756,19 @@ public:
         core_.setDistortion(d);
         return 0;
     }
+
+    // OpenCV's equidistant fisheye model (k1..k4 on theta) instead of the radial-tangential one; enabled = 0: the pinhole.  Like
+    // setDistortion, the tracker and the map restart and configure() clears it; each of the two replaces the other's model.
+    int setFisheye(int enabled, double k1, double k2, double k3, double k4) {
+        if (!configured_) { alva_set_error("System: not configured"); return ALVA_E_STATE; }
+        const double k[4] = {k1, k2, k3, k4};
+        for (double v : k)
+            if (!std::isfinite(v)) { alva_set_error("alva_system_set_fisheye: non-finite coefficient"); return ALVA_E_INVALID; }
+        if (int e = be_.set_fisheye(enabled != 0, k)) return e;
+        core_.setFisheye(enabled != 0, k);
+        return 0;
+    }
+    int lensDrops() const { return core_.n_lens_drops; }
 
     // State::claheEnabled_ / claheContrastLimit_ / claheTileSize_ and VisualFrontend's grid Size(imgWidth_ / tile, imgHeight_ / tile)
     // (visual_frontend.cpp:16-18: a double division, truncated); configure() turns it off again (system.cpp:17)
@@ -930,6 +964,11 @@ extern "C" int alva_system_set_distortion(alva_system* s, double k1, double k2, 
     if (!s) { alva_set_error("alva_system_set_distortion: null handle"); return ALVA_E_INVALID; }
     return s->sys.setDistortion(k1, k2, p1, p2);
 }
+extern "C" int alva_system_set_fisheye(alva_system* s, int enabled, double k1, double k2, double k3, double k4) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
+    if (!s) { alva_set_error("alva_system_set_fisheye: null handle"); return ALVA_E_INVALID; }
+    return s->sys.setFisheye(enabled, k1, k2, k3, k4);
+}
+extern "C" int alva_system_lens_drops(alva_system* s) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1); return s ? s->sys.lensDrops() : ALVA_E_INVALID; }
 extern "C" int alva_system_set_preset(alva_system* s, int preset) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
     if (!s) { alva_set_error("alva_system_set_preset: null handle"); return ALVA_E_INVALID; }
     return s->sys.setPreset(preset);

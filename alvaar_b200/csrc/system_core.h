@@ -149,14 +149,28 @@ struct Se3 {
 struct Camera {
     double fx = 1, fy = 1, cx = 0, cy = 0;
     int w = 0, h = 0;
-    // lens distortion k1 k2 p1 p2 (CameraCalibration::D_); has_dist = any of them non-zero.  Without it the two functions that
-    // apply it below take their pinhole forms, which give the same bits as the radial-tangential model with zero coefficients.
+    // The lens model, explicit: the pinhole, OpenCV's radial-tangential model (k1 k2 p1 p2, CameraCalibration::D_) or OpenCV's
+    // equidistant fisheye model (k1 k2 k3 k4 on theta).  has_dist = a model other than the pinhole is applied.  The
+    // radial-tangential model with all coefficients zero is the pinhole: the two functions that apply it below then take their
+    // pinhole forms, which give the same bits.  A fisheye lens with zero coefficients is the equidistant projection, not the
+    // pinhole, so the model is never inferred from the coefficients.
+    enum Lens { PINHOLE = 0, RADTAN = 1, FISHEYE = 2 };
+    int lens = PINHOLE;
     double dist[4] = {0, 0, 0, 0};
     bool has_dist = false;
     void setDistortion(const double* d) {
         has_dist = false;
         for (int i = 0; i < 4; i++) { dist[i] = d[i]; has_dist = has_dist || d[i] != 0.0; }
+        lens = has_dist ? RADTAN : PINHOLE;
     }
+    void setFisheye(bool on, const double* k) {
+        for (int i = 0; i < 4; i++) dist[i] = on ? k[i] : 0.0;
+        lens = on ? FISHEYE : PINHOLE;
+        has_dist = on;
+    }
+    // the value cv::fisheye::undistortPoints returns for a pixel it cannot undistort (Newton did not converge, or theta flipped):
+    // 1e6 px outside any image, never the result of the radial-tangential model or of a converged fisheye point in practice
+    static bool lensFailure(float ux, float uy) { return ux == -1000000.0f && uy == -1000000.0f; }
     void K4(double* k) const { k[0] = fx; k[1] = fy; k[2] = cx; k[3] = cy; }
     // CameraCalibration::undistortImagePoint: cv::undistortPoints(..., K, D, K) (camera_model.h); with zero distortion it
     // evaluates fx * ((u - cx) * (1 / fx)) + cx in double and rounds to float (calib3d/src/undistort.dispatch.cpp)
@@ -167,6 +181,14 @@ struct Camera {
         k00 = fy * id; k02 = (-(cx * fy)) * id; k11 = fx * id; k12 = (-(fx * cy)) * id; k22 = (fx * fy) * id;
     }
     void undistort(float u, float v, float& ux, float& uy) const {
+        if (lens == FISHEYE) {
+            double k[4];
+            float o[2];
+            K4(k);
+            alva_cam::undistort_point_fisheye(k, dist, u, v, o);
+            ux = o[0]; uy = o[1];
+            return;
+        }
         if (has_dist) {
             double k[4];
             float o[2];
@@ -198,6 +220,14 @@ struct Camera {
         u = (float)(fx * (p[0] * iz) + cx); v = (float)(fy * (p[1] * iz) + cy);
     }
     void projCamToImageDist(const double* p, float& u, float& v) const {   // :34-55: cv::projectPoints on a FLOAT point
+        if (lens == FISHEYE) {
+            double k[4];
+            float o[2];
+            K4(k);
+            alva_cam::project_dist_fisheye(k, dist, p, o);
+            u = o[0]; v = o[1];
+            return;
+        }
         if (has_dist) {
             double k[4];
             float o[2];
@@ -475,6 +505,7 @@ struct MatchProblem {   // Mapper::matchToMap on flat arrays (the contract of al
     std::vector<uint8_t> desc;
     std::vector<int32_t> local_mp;      // table indices of the local map, in the set's iteration order
     bool has_dist = false;              // lens distortion of the projections (Camera::dist)
+    bool fisheye = false;               // ... through the equidistant fisheye model instead of the radial-tangential one
     double dist[4] = {0, 0, 0, 0};
 };
 // the map a lost frame is matched against: every map point that is 3-D and has a descriptor, in ascending id order; its
@@ -527,6 +558,7 @@ public:
         cam.prepare();
         const double zero[4] = {0, 0, 0, 0};
         cam.setDistortion(zero);
+        n_lens_drops = 0;
         setPreset(40, 0.95f, true);   // State(w, h, 40), mapKeyframeFilteringRatio_ 0.95, p3pEnabled_ (system.cpp:15-19)
         reloc_max = 0;
     }
@@ -550,6 +582,13 @@ public:
     // the lens model of every later frame; the map and the tracked keypoints were made under the previous one: reset
     void setDistortion(const double* d) {
         cam.setDistortion(d);
+        n_lens_drops = 0;
+        reset();
+    }
+    // the equidistant fisheye model (on = false: the pinhole); replaces the radial-tangential model and is replaced by it
+    void setFisheye(bool on, const double* k) {
+        cam.setFisheye(on, k);
+        n_lens_drops = 0;
         reset();
     }
 
@@ -715,6 +754,9 @@ public:
     int n_pnp_prior = 0, n_p3p_fallback = 0, n_local_ba = 0, n_free_pose_clamp = 0;
     // relocalisation: times the track was lost, frames relocalised, and the matches / PnP inliers of the last attempt
     int n_lost = 0, n_relocalised = 0, reloc_last_matches = 0, reloc_last_inliers = 0;
+    // keypoints dropped because the fisheye model could not undistort them (tracked, detected or relocalisation queries), since
+    // configure or the last lens change
+    int n_lens_drops = 0;
 
 private:
     Backend& B;
@@ -808,6 +850,7 @@ private:
                 if ((err = B.describe(fresh.data(), nn, desc.data(), kept.data())) < 0) return;
                 err = 0;
                 for (int i = 0; i < nn; i++) {   // addKeypointsToFrame + addMapPoint (map_manager.cpp:152-191, 255-330)
+                    if (lensDrop(fresh[2 * i], fresh[2 * i + 1], un ? &fresh_un[2 * (size_t)i] : nullptr)) continue;
                     const uint8_t* d = kept[i] ? &desc[32 * (size_t)i] : nullptr;
                     cur.add(fresh[2 * i], fresh[2 * i + 1], n_mp_ids, d, un ? &fresh_un[2 * (size_t)i] : nullptr);
                     MapPoint mp;
@@ -922,6 +965,7 @@ private:
         frame.Twc.to7(m.Twc_cur);
         m.nkp3d = frame.n3d;
         m.has_dist = cam.has_dist;
+        m.fisheye = cam.lens == Camera::FISHEYE;
         for (int i = 0; i < 4; i++) m.dist[i] = cam.dist[i];
         // the frame's keypoints cell by cell, each cell in its insertion order (what Frame::getSurroundingKeypoints walks)
         std::unordered_map<int, int> mp_index;
@@ -1302,6 +1346,7 @@ private:
         std::vector<double> qbv, quv;
         for (int i = 0; i < nn; i++) {
             if (!kept[i]) continue;
+            if (lensDrop(fresh[2 * i], fresh[2 * i + 1], un ? &fresh_un[2 * (size_t)i] : nullptr)) continue;
             Keypoint k;
             cur.compute(fresh[2 * i], fresh[2 * i + 1], k, un ? &fresh_un[2 * (size_t)i] : nullptr);
             memcpy(k.desc, &desc[32 * (size_t)i], 32);
@@ -1384,6 +1429,7 @@ private:
             const float* un = backendUnpx();
             size_t ngood = 0;
             for (size_t i = 0; i < n3; i++) {
+                if (good[i] && lensDrop(pri3[2 * i], pri3[2 * i + 1], un ? un + 2 * i : nullptr)) { removeObsFromCurr(ids3[i]); continue; }
                 if (good[i]) { cur.update(ids3[i], pri3[2 * i], pri3[2 * i + 1], un ? un + 2 * i : nullptr); ngood++; }
                 else { ids.push_back(ids3[i]); kps.push_back(kps3[2 * i]); kps.push_back(kps3[2 * i + 1]); pri.push_back(pri3[2 * i]); pri.push_back(pri3[2 * i + 1]); }
             }
@@ -1396,10 +1442,23 @@ private:
             err = 0;
             const float* un = backendUnpx();
             for (size_t i = 0; i < n; i++) {
-                if (good[i]) cur.update(ids[i], pri[2 * i], pri[2 * i + 1], un ? un + 2 * i : nullptr);
+                if (good[i] && !lensDrop(pri[2 * i], pri[2 * i + 1], un ? un + 2 * i : nullptr)) cur.update(ids[i], pri[2 * i], pri[2 * i + 1], un ? un + 2 * i : nullptr);
                 else removeObsFromCurr(ids[i]);
             }
         }
+    }
+
+    // A keypoint at (x, y) whose fisheye undistortion fails is dropped, the same way whichever side undistorted it (un: the
+    // backend's result, else Camera::undistort): a tracked point is removed as a KLT failure, a detected point or a
+    // relocalisation query is never added.  Counted in n_lens_drops.  Never true for the pinhole or radial-tangential lens.
+    bool lensDrop(float x, float y, const float* un) {
+        if (cam.lens != Camera::FISHEYE) return false;
+        float ux, uy;
+        if (un) { ux = un[0]; uy = un[1]; }
+        else cam.undistort(x, y, ux, uy);
+        if (!Camera::lensFailure(ux, uy)) return false;
+        n_lens_drops++;
+        return true;
     }
 
     // the undistorted positions of the points the last klt() / detect() returned, when the backend computed them

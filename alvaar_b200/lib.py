@@ -68,6 +68,10 @@ _OPTIONAL = {
                                  _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, C.c_float, C.c_float, _vp, _vp, _vp, _vp],
     "alva_k_undistort_points": [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp],
     "alva_k_project_points": [_vp, _vp, _i32, _vp, _vp, _vp],
+    "alva_k_match_to_map_fisheye": [_vp, _i32, _i32, _i32, C.c_double, C.c_double, C.c_double, C.c_double, _vp, _i32, _vp, _vp, _i32, _i32,
+                                    _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, C.c_float, C.c_float, _vp, _vp, _vp, _vp],
+    "alva_k_undistort_points_fisheye": [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp],
+    "alva_k_project_points_fisheye": [_vp, _vp, _i32, _vp, _vp, _vp],
     "alva_k_p3p_lmeds": [_vp, _i32, _i32, _vp, _vp, _vp, _i32, C.c_float, C.c_float, C.c_float, C.c_uint32, _vp, _vp, _vp],
     "alva_k_p3p_ransac": [_vp, _i32, _i32, _vp, _vp, _vp, _i32, C.c_float, C.c_float, C.c_float, C.c_uint32, _vp, _vp, _vp],
     "alva_k_hamming_knn2_grouped": [_vp, _vp, _i32, _vp, _i32, _vp, _i32, _vp],
@@ -223,14 +227,19 @@ class Context:
         self._chk(self.L.alva_k_corner_subpix(self.h, _ptr(gray), w, h, nframes, _ptr(pts), _ptr(counts), cap))
 
     def match_to_map(self, w, h, cell, K, Twc_cur, kp_mp, kp_px, nkp3d, kf_Twc, mp_wpt, mp_is3d, obs_start, obs_kf, obs_px,
-                     desc_start, desc, local_mp, kp_match, kp_dist, n_match, max_proj_err=2.0, dist_ratio=0.2, dist=None):
+                     desc_start, desc, local_mp, kp_match, kp_dist, n_match, max_proj_err=2.0, dist_ratio=0.2, dist=None, fisheye=None):
         """Mapper::matchToMap on flat device arrays -- see alva_k_match_to_map; dist = (k1, k2, p1, p2): the lens-distorted
-        projections of alva_k_match_to_map_dist."""
+        projections of alva_k_match_to_map_dist; fisheye = (k1, k2, k3, k4): those of the equidistant fisheye model
+        (alva_k_match_to_map_fisheye)."""
         args = (self.h, w, h, cell, K[0], K[1], K[2], K[3], _ptr(Twc_cur), kp_mp.numel(), _ptr(kp_mp), _ptr(kp_px), nkp3d,
                 kf_Twc.shape[0], _ptr(kf_Twc), mp_wpt.shape[0], _ptr(mp_wpt), _ptr(mp_is3d), _ptr(obs_start), _ptr(obs_kf),
                 _ptr(obs_px), _ptr(desc_start), _ptr(desc), local_mp.numel(), _ptr(local_mp), max_proj_err, dist_ratio,
                 _ptr(kp_match), _ptr(kp_dist), _ptr(n_match))
-        if dist is None:
+        if fisheye is not None:
+            if dist is not None:
+                raise ValueError("match_to_map: dist and fisheye are two lens models; give one")
+            self._chk(self.L.alva_k_match_to_map_fisheye(*args, _f64x4(fisheye)))
+        elif dist is None:
             self._chk(self.L.alva_k_match_to_map(*args))
         else:
             self._chk(self.L.alva_k_match_to_map_dist(*args, _f64x4(dist)))
@@ -244,6 +253,15 @@ class Context:
         """CameraCalibration::projectCamToImageDist of n camera-frame points Xc [n][3] float64 into uv [n][2] float32 -- see
         alva_k_project_points."""
         self._chk(self.L.alva_k_project_points(self.h, _ptr(Xc), n, _f64x4(K), _f64x4(dist), _ptr(uv)))
+
+    def undistort_points_fisheye(self, px, counts, nframes, cap, K, k4, unpx):
+        """cv::fisheye::undistortPoints(px, unpx, K, D, noArray(), K) -- see alva_k_undistort_points_fisheye; k4 = (k1, k2, k3, k4).
+        Points the model cannot undistort come back as (-1e6, -1e6)."""
+        self._chk(self.L.alva_k_undistort_points_fisheye(self.h, _ptr(px), _ptr(counts), nframes, cap, _f64x4(K), _f64x4(k4), _ptr(unpx)))
+
+    def project_points_fisheye(self, Xc, n, K, k4, uv):
+        """cv::fisheye::projectPoints of the float points (x/z, y/z, 1) -- see alva_k_project_points_fisheye."""
+        self._chk(self.L.alva_k_project_points_fisheye(self.h, _ptr(Xc), n, _f64x4(K), _f64x4(k4), _ptr(uv)))
 
     def p3p_lmeds(self, nprob, cap, bvs, wpts, counts, Twc_out, outlier, info=None, max_iter=100, err_px=3.0, fx=1.0, fy=1.0,
                   seed=12345):

@@ -5,7 +5,7 @@
             1280x720 view, so 1000 features/frame is always reachable.
 * frames  : a pinhole camera on a smooth seeded SE(3) trajectory (about 3 px/frame lateral motion, +-0.2 deg/frame
             rotation) looking at the texture plane z = 4; bilinear sampling; RGBA with R = G = B, A = 255.  Optionally
-            through OpenCV's radial-tangential lens (k1, k2, p1, p2).
+            through OpenCV's radial-tangential lens (k1, k2, p1, p2) or its equidistant fisheye lens (k1, k2, k3, k4).
 * descriptors / BA problems for the matcher and bundle-adjustment stages.
 Pure numpy (+ scipy.ndimage for the blur); nothing here is on the product path.
 """
@@ -81,14 +81,39 @@ def undistort_normalised(xd, yd, dist, tol=1e-12, max_iter=500):
     raise ValueError(f"lens model {dist} does not invert over this image")
 
 
-def render_gray(tex, pose, w, h, plane_z=4.0, tex_scale=None, dist=None):
-    """Bilinear render of the texture plane z = plane_z seen from pose (R_wc, t_wc); dist = (k1, k2, p1, p2): through that lens."""
+def fisheye_theta(theta_d, k, tol=1e-14, max_iter=200):
+    """The incidence angle theta that OpenCV's equidistant fisheye model (k1, k2, k3, k4) maps to theta_d = theta (1 + k1 theta^2
+    + k2 theta^4 + k3 theta^6 + k4 theta^8): Newton's method run to convergence (scene generation, not cv::fisheye's 10 steps)."""
+    k1, k2, k3, k4 = k
+    th = theta_d.copy()
+    for _ in range(max_iter):
+        t2 = th * th
+        f = th * (1 + t2 * (k1 + t2 * (k2 + t2 * (k3 + t2 * k4)))) - theta_d
+        df = 1 + t2 * (3 * k1 + t2 * (5 * k2 + t2 * (7 * k3 + t2 * 9 * k4)))
+        step = f / df
+        th = th - step
+        if np.abs(step).max() < tol:
+            if (th < 0).any() or (th >= np.pi / 2).any():
+                break
+            return th
+    raise ValueError(f"fisheye model {k} does not invert over this image below 90 degrees")
+
+
+def render_gray(tex, pose, w, h, plane_z=4.0, tex_scale=None, dist=None, fisheye=None):
+    """Bilinear render of the texture plane z = plane_z seen from pose (R_wc, t_wc); dist = (k1, k2, p1, p2): through that lens;
+    fisheye = (k1, k2, k3, k4): through OpenCV's equidistant fisheye lens instead."""
     fx, fy, cx, cy = intrinsics(w, h)
     if tex_scale is None:
         tex_scale = fx / plane_z          # texture pixels per world unit: ~1 texel per image pixel
     R, t = pose
     u, v = np.meshgrid(np.arange(w, dtype=np.float64), np.arange(h, dtype=np.float64))
-    if dist is None:
+    if fisheye is not None:
+        xd, yd = (u - cx) / fx, (v - cy) / fy
+        theta_d = np.sqrt(xd * xd + yd * yd)
+        theta = fisheye_theta(theta_d, fisheye)
+        scale = np.where(theta_d > 0, np.tan(theta) / np.where(theta_d > 0, theta_d, 1.0), 1.0)
+        rays = np.stack([xd * scale, yd * scale, np.ones_like(u)], -1) @ R.T
+    elif dist is None:
         rays = np.stack([(u - cx) / fx, (v - cy) / fy, np.ones_like(u)], -1) @ R.T
     else:
         x, y = undistort_normalised((u - cx) / fx, (v - cy) / fy, dist)
@@ -119,12 +144,15 @@ def gray_to_rgba(g):
     return out
 
 
-def make_frames(nframes, w, h, seed=99, rgba=True, texture_seed=1234, dist=None):
+def make_frames(nframes, w, h, seed=99, rgba=True, texture_seed=1234, dist=None, fisheye=None):
     """`seed` picks the camera path, `texture_seed` the scene (two calls with the same texture_seed look at the same plane);
-    dist = (k1, k2, p1, p2) renders through OpenCV's radial-tangential lens with the intrinsics() camera (None: a pinhole)."""
+    dist = (k1, k2, p1, p2) renders through OpenCV's radial-tangential lens with the intrinsics() camera (None: a pinhole);
+    fisheye = (k1, k2, k3, k4) through OpenCV's equidistant fisheye lens with the same camera matrix."""
+    if dist is not None and fisheye is not None:
+        raise ValueError("make_frames: dist and fisheye are two lens models; give one")
     tex = make_texture(seed=texture_seed)
     poses = trajectory(nframes, w, h, seed)
-    frames = [render_gray(tex, p, w, h, dist=dist) for p in poses]
+    frames = [render_gray(tex, p, w, h, dist=dist, fisheye=fisheye) for p in poses]
     g = np.stack(frames)
     return (gray_to_rgba(g) if rgba else g), poses
 

@@ -19,6 +19,8 @@ def _bind():
     L.alva_system_reset.argtypes = [_vp]
     L.alva_system_set_clahe.argtypes = [_vp, _i32, _f64, _i32]
     L.alva_system_set_distortion.argtypes = [_vp] + [_f64] * 4
+    L.alva_system_set_fisheye.argtypes = [_vp, _i32] + [_f64] * 4
+    L.alva_system_lens_drops.argtypes = [_vp]
     L.alva_system_set_preset.argtypes = [_vp, _i32]
     L.alva_system_set_relocalisation.argtypes = [_vp, _i32]
     L.alva_system_num_matched.argtypes = [_vp]
@@ -157,6 +159,20 @@ class System:
         rc = self.L.alva_system_set_distortion(self.h, float(k1), float(k2), float(p1), float(p2))
         if rc != 0:
             raise AlvaError(f"alva_system_set_distortion -> {rc}: {self.L.alva_last_error().decode()}")
+
+    def set_fisheye(self, enabled, k1=0.0, k2=0.0, k3=0.0, k4=0.0):
+        """OpenCV's equidistant fisheye lens (cv::fisheye, k1..k4 on the incidence angle) for wide-angle cameras: keypoints are
+        undistorted with cv::fisheye::undistortPoints, projections use cv::fisheye::projectPoints.  enabled=False returns to the
+        pinhole; zero coefficients with enabled=True are the equidistant projection.  Replaces set_distortion's model (and is
+        replaced by it); resets the tracker and the map; survives reset() and set_preset(); configuring clears it.  Keypoints
+        the model cannot undistort are dropped (lens_drops())."""
+        rc = self.L.alva_system_set_fisheye(self.h, 1 if enabled else 0, float(k1), float(k2), float(k3), float(k4))
+        if rc != 0:
+            raise AlvaError(f"alva_system_set_fisheye -> {rc}: {self.L.alva_last_error().decode()}")
+
+    def lens_drops(self):
+        """keypoints dropped because the fisheye model could not undistort them, since configuring or the last lens change"""
+        return int(self.L.alva_system_lens_drops(self.h))
 
     def set_relocalisation(self, max_lost_frames):
         """Relocalise against the kept map after a tracking loss instead of discarding it.  0 (the default) is the reference's

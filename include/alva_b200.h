@@ -96,6 +96,18 @@ int alva_k_clahe(alva_ctx*, const uint8_t* src, uint8_t* dst, int w, int h, int 
 int alva_k_undistort_points(alva_ctx*, const float* px, const int32_t* counts, int nframes, int cap, const double* K4,
                             const double* D4, float* unpx);
 int alva_k_project_points(alva_ctx*, const double* Xc, int n, const double* K4, const double* D4, float* uv);
+/* The same two calls through OpenCV's equidistant fisheye model (cv::fisheye, "Kannala-Brandt"), D4 = {k1, k2, k3, k4} on the
+ * incidence angle theta: theta_d = theta (1 + k1 theta^2 + k2 theta^4 + k3 theta^6 + k4 theta^8).  Same shapes, layout, counts
+ * and argument checks as above; zero coefficients are the equidistant projection, not the pinhole.
+ * alva_k_undistort_points_fisheye: cv::fisheye::undistortPoints(px, unpx, K, D, noArray(), K) -- theta_d clamped to
+ * [-pi/2, pi/2], at most 10 Newton steps (stop at |step| < 1e-8), the result in pixels of the same K; (-1e6, -1e6) where the
+ * iteration does not converge or theta changes sign.
+ * alva_k_project_points_fisheye: cv::fisheye::projectPoints of the float point (x/z, y/z, 1), zero rvec / tvec, alpha 0.
+ * Bit-exact with the library up to atan / tan, which here are one deterministic double version on host and device (a float
+ * result can differ from a glibc build only where its double lies within a few ulps of a float rounding boundary). */
+int alva_k_undistort_points_fisheye(alva_ctx*, const float* px, const int32_t* counts, int nframes, int cap, const double* K4,
+                                    const double* D4, float* unpx);
+int alva_k_project_points_fisheye(alva_ctx*, const double* Xc, int n, const double* K4, const double* D4, float* uv);
 
 /* cv::FAST(gray, thr, nms=true, TYPE_9_16) on each frame (opencv features2d/src/fast.cpp:496).
  * keys[f*cap + i]: packed corner keys; counts[f] = true number found (may exceed cap: then only cap
@@ -295,6 +307,15 @@ int alva_k_match_to_map_dist(alva_ctx*, int w, int h, int cell, double fx, doubl
                              const float* obs_px, const int32_t* desc_start, const uint8_t* desc, int n_local, const int32_t* local_mp,
                              float max_proj_err, float dist_ratio, int32_t* kp_match, float* kp_dist, int32_t* n_match,
                              const double* dist4);
+/* The same through the equidistant fisheye model: fisheye4 = {k1, k2, k3, k4} (HOST array, required; zeros are a valid lens)
+ * projects the map point and the co-projection errors as alva_k_project_points_fisheye does.  ALVA_E_INVALID for a NULL or
+ * non-finite fisheye4. */
+int alva_k_match_to_map_fisheye(alva_ctx*, int w, int h, int cell, double fx, double fy, double cx, double cy, const double* Twc_cur,
+                                int n_kp, const int32_t* kp_mp, const float* kp_px, int nkp3d, int n_kf, const double* kf_Twc, int n_mp,
+                                const double* mp_wpt, const uint8_t* mp_is3d, const int32_t* obs_start, const int32_t* obs_kf,
+                                const float* obs_px, const int32_t* desc_start, const uint8_t* desc, int n_local, const int32_t* local_mp,
+                                float max_proj_err, float dist_ratio, int32_t* kp_match, float* kp_dist, int32_t* n_match,
+                                const double* fisheye4);
 
 /* Local bundle adjustment, batched over nprob independent problems of identical dimensions
  * (Optimizer::localBA, src/slam/src/optimizer.cpp:4-531, solved the way ceres::Solve does with the reference's
@@ -452,6 +473,20 @@ int  alva_system_set_clahe(alva_system*, int enabled, double clip_limit, int til
  * reset() does; the next frame starts under the new model.  All zero = the pinhole camera.  configure clears it, reset keeps it.
  * ALVA_E_STATE before configure; ALVA_E_INVALID for a null handle or a non-finite coefficient. */
 int  alva_system_set_distortion(alva_system*, double k1, double k2, double p1, double p2);
+/* The equidistant fisheye lens of a configured System (OpenCV's cv::fisheye, k1..k4 on theta): the wide-angle cameras the
+ * radial-tangential model cannot describe.  enabled = 1 selects it, with any finite coefficients (zeros are the equidistant
+ * projection); enabled = 0 returns to the pinhole.  It is applied where set_distortion's model is -- tracked and detected
+ * keypoints are undistorted on the device with cv::fisheye::undistortPoints, the KLT priors of 3-D keypoints and the local-map
+ * matcher project with cv::fisheye::projectPoints -- and everything downstream works on undistorted pixels.  A keypoint the
+ * model cannot undistort (OpenCV's (-1e6, -1e6)) is dropped: a tracked one as a KLT failure, a detected one is never added;
+ * alva_system_lens_drops counts them.  set_distortion and set_fisheye each replace the other's model.  It resets the tracker and
+ * the map as reset() does; configure clears it; reset, set_preset, set_clahe and set_relocalisation keep it.  ALVA_E_STATE
+ * before configure; ALVA_E_INVALID for a null handle or a non-finite coefficient.  Fields of view of 180 degrees or more are
+ * out of its range (OpenCV clamps theta_d to pi/2). */
+int  alva_system_set_fisheye(alva_system*, int enabled, double k1, double k2, double k3, double k4);
+/* keypoints dropped because the fisheye model could not undistort them, since configure or the last set_distortion /
+ * set_fisheye (always 0 for the pinhole and radial-tangential lenses) */
+int  alva_system_lens_drops(alva_system*);
 /* The reference's three tuned configurations (state.hpp:9-17), and DEFAULT = what configure sets (system.cpp:15-19):
  *              grid cell  CLAHE (clip 3, tile 50)  keyframe filtering ratio  P3P on every tracked frame
  *   DEFAULT    40 px      off                      0.95                      yes

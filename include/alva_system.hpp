@@ -34,6 +34,9 @@ public:
     // not in the reference's class: relocalise for up to maxLostFrames frames after a tracking loss instead of resetting
     // (findCameraPose then returns ALVA_STATUS_LOST while lost; 0 = the reference's reset); 0 or an ALVA_E_* code
     int setRelocalisation(int maxLostFrames) { return alva_system_set_relocalisation(h_, maxLostFrames); }
+    // not in the reference's class: OpenCV's equidistant fisheye lens (k1..k4 on theta; enabled = 0: the pinhole), for
+    // wide-angle cameras; resets the tracker and the map; 0 or an ALVA_E_* code
+    int setFisheye(int enabled, double k1, double k2, double k3, double k4) { return alva_system_set_fisheye(h_, enabled, k1, k2, k3, k4); }
 
     // ---- the reference's wasm32 signatures
     int findCameraPose(int imageRGBADataPtr, int posePtr) { return findCameraPose(ptr<const uint8_t>(imageRGBADataPtr), ptr<float>(posePtr)); }
