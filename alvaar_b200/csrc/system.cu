@@ -882,6 +882,24 @@ public:
         core_.setRelocalisation(max_lost_frames);
         return 0;
     }
+    // The map blob (system_core.h: saveMap / loadMap).  Nothing on the device holds the map itself: the relocalisation table
+    // is re-uploaded because a load bumps RelocTable::version (reset() and the table build both do), the local-map matcher
+    // uploads its problem on every call, and the previous pyramid is not read before the relocalised frame rewrites it.
+    int saveMap(uint8_t* buf, size_t cap, size_t* bytes) {
+        if (!configured_) { alva_set_error("System: not configured"); return ALVA_E_STATE; }
+        std::vector<uint8_t> blob;
+        if (int e = core_.saveMap(blob)) { alva_set_error("alva_system_save_map: %s", core_.map_error); return e; }
+        *bytes = blob.size();
+        if (!buf) return 0;
+        if (cap < blob.size()) { alva_set_error("alva_system_save_map: the map needs %zu bytes, the buffer holds %zu", blob.size(), cap); return ALVA_E_CAPACITY; }
+        memcpy(buf, blob.data(), blob.size());
+        return 0;
+    }
+    int loadMap(const uint8_t* buf, size_t bytes) {
+        if (!configured_) { alva_set_error("System: not configured"); return ALVA_E_STATE; }
+        if (int e = core_.loadMap(buf, bytes)) { alva_set_error("alva_system_load_map: %s", core_.map_error); return e; }
+        return 0;
+    }
     // page-lock a caller-owned frame buffer that is reused from call to call (the reference's shim allocates its image buffer once,
     // system.js:63-67): uploads from it then run at the host link's rate instead of through the driver's pageable staging
     int pinBuffer(void* ptr, size_t bytes) {
@@ -976,6 +994,14 @@ extern "C" int alva_system_set_preset(alva_system* s, int preset) { AlvaDeviceGu
 extern "C" int alva_system_set_relocalisation(alva_system* s, int max_lost_frames) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
     if (!s || max_lost_frames < 0) { alva_set_error("alva_system_set_relocalisation: bad argument"); return ALVA_E_INVALID; }
     return s->sys.setRelocalisation(max_lost_frames);
+}
+extern "C" int alva_system_save_map(alva_system* s, uint8_t* buf, size_t cap, size_t* bytes) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
+    if (!s || !bytes) { alva_set_error("alva_system_save_map: bad argument"); return ALVA_E_INVALID; }
+    return s->sys.saveMap(buf, cap, bytes);
+}
+extern "C" int alva_system_load_map(alva_system* s, const uint8_t* buf, size_t bytes) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
+    if (!s || !buf) { alva_set_error("alva_system_load_map: bad argument"); return ALVA_E_INVALID; }
+    return s->sys.loadMap(buf, bytes);
 }
 extern "C" int alva_system_reset(alva_system* s) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1); if (!s) return ALVA_E_INVALID; s->sys.reset(); return 0; }
 extern "C" int alva_system_find_camera_pose(alva_system* s, const uint8_t* rgba, float* pose16) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);

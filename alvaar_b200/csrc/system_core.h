@@ -528,6 +528,40 @@ struct RelocResult {
     std::vector<uint8_t> o1, o2;
 };
 
+// ------------------------------------------------------------------------------------------------ map blob byte order
+// fixed-width little-endian fields, no padding (a little-endian host is assumed: x86-64 and aarch64 Linux)
+static_assert(sizeof(float) == 4 && sizeof(double) == 8, "the map blob stores IEEE binary32 / binary64");
+struct MapWriter {
+    std::vector<uint8_t>& o;
+    explicit MapWriter(std::vector<uint8_t>& out) : o(out) { o.clear(); }
+    void raw(const void* p, size_t n) { const uint8_t* b = (const uint8_t*)p; o.insert(o.end(), b, b + n); }
+    void u8(uint8_t v) { o.push_back(v); }
+    void i32(int32_t v) { raw(&v, 4); }
+    void u32(uint32_t v) { raw(&v, 4); }
+    void u64(uint64_t v) { raw(&v, 8); }
+    void f32(float v) { raw(&v, 4); }
+    void f64(double v) { raw(&v, 8); }
+    void se3(const Se3& T) { for (int i = 0; i < 3; i++) f64(T.t[i]); for (int i = 0; i < 4; i++) f64(T.q[i]); }
+};
+// every read is bounds-checked: false (and nothing read) past the end
+struct MapReader {
+    const uint8_t* p;
+    size_t n, off = 0;
+    MapReader(const uint8_t* d, size_t bytes) : p(d), n(bytes) {}
+    size_t left() const { return n - off; }
+    bool raw(void* dst, size_t k) { if (k > left()) return false; memcpy(dst, p + off, k); off += k; return true; }
+    bool u8(uint8_t& v) { return raw(&v, 1); }
+    bool flag(bool& v) { uint8_t b; if (!u8(b) || b > 1) return false; v = b != 0; return true; }   // 0 or 1 only
+    bool i32(int32_t& v) { return raw(&v, 4); }
+    bool u32(uint32_t& v) { return raw(&v, 4); }
+    bool u64(uint64_t& v) { return raw(&v, 8); }
+    bool f32(float& v) { return raw(&v, 4) && std::isfinite(v); }   // finite values only
+    bool f64(double& v) { return raw(&v, 8) && std::isfinite(v); }
+    bool se3(Se3& T) { for (int i = 0; i < 3; i++) if (!f64(T.t[i])) return false; for (int i = 0; i < 4; i++) if (!f64(T.q[i])) return false; return true; }
+    // a count of records of at least `min_bytes` each that the rest of the blob can hold
+    bool count(uint32_t& c, size_t min_bytes) { return u32(c) && (uint64_t)c * min_bytes <= left(); }
+};
+
 // ------------------------------------------------------------------------------------------------ the state machine
 // Backend concept (host pointers in, host pointers out; < 0 = ALVA_E_* error):
 //   int pyramid(const uint8_t* rgba)                       gray + pyramid + Scharr levels of the new frame; previous <- current
@@ -601,6 +635,97 @@ public:
         lost = false; lost_frames = 0;
         reloc_table.clear();
         // VisualFrontend::reset leaves the motion model and p3pReq_ alone (visual_frontend.cpp:718-728); so does this
+    }
+
+    // ------------------------------------------------------------------ the map blob (not in the reference)
+    // The layout is documented in include/alva_b200.h (alva_system_save_map) and INTEGRATION.md.  Return codes: 0, MAP_STATE
+    // (= ALVA_E_STATE) or MAP_INVALID (= ALVA_E_INVALID); map_error names the failed check.
+    enum { MAP_INVALID = -1, MAP_STATE = -4 };
+    static constexpr uint32_t MAP_VERSION = 1;
+    mutable const char* map_error = "";
+
+    // the blob of the current map; allowed once initialised (also while lost).  Reads the containers only.
+    int saveMap(std::vector<uint8_t>& out) const {
+        if (!ready_for_init) { map_error = "not initialised"; return MAP_STATE; }
+        MapWriter w(out);
+        std::vector<int> kf_ids, mp_ids;
+        for (auto& kv : keyframes) kf_ids.push_back(kv.first);
+        for (auto& kv : mappoints) mp_ids.push_back(kv.first);
+        std::sort(kf_ids.begin(), kf_ids.end());
+        std::sort(mp_ids.begin(), mp_ids.end());
+        w.raw("ALMP", 4); w.u32(MAP_VERSION); w.u64(0); w.u32((uint32_t)kf_ids.size()); w.u32((uint32_t)mp_ids.size());
+        w.i32(cam.w); w.i32(cam.h); w.f64(cam.fx); w.f64(cam.fy); w.f64(cam.cx); w.f64(cam.cy); w.i32(cam.lens);
+        for (int i = 0; i < 4; i++) w.f64(cam.dist[i]);
+        w.i32(cell);
+        w.i32(n_kf_ids); w.i32(n_mp_ids); w.i32(n_kf);
+        w.se3(cur.Twc);
+        for (int id : kf_ids) {
+            const Frame& f = *keyframes.at(id);
+            w.i32(id); w.i32(cur.id - f.id); w.se3(f.Twc);
+            std::vector<int> kp;
+            for (auto& kv : f.kps) kp.push_back(kv.first);
+            std::sort(kp.begin(), kp.end());
+            w.u32((uint32_t)kp.size());
+            for (int k : kp) {
+                const Keypoint& p = f.kps.at(k);
+                w.i32(p.id); w.f32(p.px); w.f32(p.py); w.f32(p.ux); w.f32(p.uy);
+                for (int i = 0; i < 3; i++) w.f64(p.bv[i]);
+                w.u8(p.is3d); w.u8(p.has_desc); w.raw(p.desc, 32);
+            }
+            w.u32((uint32_t)f.covis.size());
+            for (auto& kv : f.covis) { w.i32(kv.first); w.i32(kv.second); }
+            std::vector<int> lm(f.localmap.begin(), f.localmap.end());
+            std::sort(lm.begin(), lm.end());
+            w.u32((uint32_t)lm.size());
+            for (int k : lm) w.i32(k);
+        }
+        for (int id : mp_ids) {
+            const MapPoint& m = mappoints.at(id);
+            // `observed` as the lost state holds it: entering LOST clears the flag of every point of the current frame
+            w.i32(m.id); w.i32(m.kfid); w.u8(m.observed && !cur.kps.count(m.id)); w.u8(m.is3d); w.f64(m.invd);
+            for (int i = 0; i < 3; i++) w.f64(m.p[i]);
+            w.u32((uint32_t)m.obs.size());
+            for (int k : m.obs) w.i32(k);
+            std::vector<int> dk;
+            for (auto& kv : m.kfdesc) dk.push_back(kv.first);
+            std::sort(dk.begin(), dk.end());
+            w.u32((uint32_t)dk.size());
+            for (int k : dk) { w.i32(k); w.raw(m.kfdesc.at(k).b, 32); w.f32(m.descdist.at(k)); }
+            // desc_ of a point that never had a descriptor is uninitialised (and never read): zeros then
+            static const uint8_t zero[32] = {0};
+            w.u8(m.has_desc); w.raw(m.has_desc ? m.desc.b : zero, 32);
+        }
+        const uint64_t total = out.size();
+        memcpy(&out[8], &total, 8);
+        return 0;
+    }
+
+    // Replace the map with a blob's and enter the lost state: the next frames relocalise into it (status 4 while lost, 1 once
+    // relocalised, 2 after reloc_max failures).  The whole blob is parsed and checked before anything changes; a refused blob
+    // leaves the system as it was.
+    int loadMap(const uint8_t* data, size_t bytes) {
+        if (reloc_max <= 0 || !BackendHasReloc<Backend>::value) { map_error = "relocalisation is off"; return MAP_STATE; }
+        if (!data) { map_error = "null buffer"; return MAP_INVALID; }
+        LoadedMap L;
+        if (!parseMap(data, bytes, L)) return MAP_INVALID;
+        reset();
+        // fresh containers: bucket counts, and so the iteration order of what is inserted next, depend on the blob alone
+        keyframes = std::unordered_map<int, std::shared_ptr<Frame>>();
+        mappoints = std::unordered_map<int, MapPoint>();
+        cur.kps = std::unordered_map<int, Keypoint>();
+        cur.covis.clear(); cur.localmap = std::unordered_set<int>();
+        for (auto& f : L.kfs) keyframes.emplace(f->kfid, f);
+        for (auto& m : L.mps) mappoints.emplace(m.id, std::move(m));
+        n_kf_ids = L.n_kf_ids; n_mp_ids = L.n_mp_ids; n_kf = L.n_kf;
+        ready_for_init = true;
+        motion.reset();
+        p3p_req = true;
+        cur.kfid = n_kf_ids > 0 ? n_kf_ids - 1 : 0;   // createKeyframe's; the newest keyframe is never filtered out
+        cur.setTwc(L.pose);
+        buildRelocTable();
+        lost = true;
+        lost_frames = 0;
+        return 0;
     }
 
     // System::processCameraPose: returns 1 tracking / 2 reset / 3 not initialised / 4 lost (relocalisation on), or a negative
@@ -763,6 +888,160 @@ private:
     MotionModel motion;
     bool p3p_req = false;
     int pose_failed = 0, err = 0;
+
+    // ------------------------------------------------------------------ map blob parsing: nothing of the system is touched
+    struct LoadedMap {
+        std::vector<std::shared_ptr<Frame>> kfs;    // ascending id
+        std::vector<MapPoint> mps;                  // ascending id
+        int n_kf_ids = 0, n_mp_ids = 0, n_kf = 0;
+        Se3 pose;
+    };
+    // every rotation the state machine stores went through Se3::normalize (or exp's sin / cos): unit up to rounding
+    static bool unitQuat(const Se3& T) {
+        const double n2 = T.q[0] * T.q[0] + T.q[1] * T.q[1] + T.q[2] * T.q[2] + T.q[3] * T.q[3];
+        return fabs(n2 - 1.0) <= 1e-9;
+    }
+    bool parseMap(const uint8_t* data, size_t bytes, LoadedMap& L) {
+        auto fail = [this](const char* why) { map_error = why; return false; };
+        MapReader r(data, bytes);
+        char magic[4];
+        uint32_t version = 0, nkf = 0, nmp = 0;
+        uint64_t total = 0;
+        if (!r.raw(magic, 4) || memcmp(magic, "ALMP", 4) != 0) return fail("bad magic");
+        if (!r.u32(version) || version != MAP_VERSION) return fail("unsupported version");
+        if (!r.u64(total) || total != (uint64_t)bytes) return fail("byte count differs from the blob's length");
+        if (!r.u32(nkf) || !r.u32(nmp)) return fail("truncated header");
+        int32_t w = 0, h = 0, lens = 0, cs = 0;
+        double K[4], D[4];
+        bool ok = r.i32(w) && r.i32(h);
+        for (int i = 0; i < 4; i++) ok = ok && r.f64(K[i]);
+        ok = ok && r.i32(lens);
+        for (int i = 0; i < 4; i++) ok = ok && r.f64(D[i]);
+        if (!ok) return fail("truncated or non-finite camera section");
+        bool same = w == cam.w && h == cam.h && K[0] == cam.fx && K[1] == cam.fy && K[2] == cam.cx && K[3] == cam.cy && lens == cam.lens;
+        for (int i = 0; i < 4; i++) same = same && D[i] == cam.dist[i];
+        if (!same) return fail("camera or lens differs from the configured one");
+        if (!r.i32(cs)) return fail("truncated grid section");
+        if (cs != cell) return fail("grid cell size differs from the preset's");
+        if (!r.i32(L.n_kf_ids) || !r.i32(L.n_mp_ids) || !r.i32(L.n_kf)) return fail("truncated counters");
+        // below 2^30: the counters keep growing after the load and must not overflow
+        auto counter_ok = [](int v) { return v >= 0 && v <= (1 << 30); };
+        if (!counter_ok(L.n_kf_ids) || !counter_ok(L.n_mp_ids) || L.n_kf != (int64_t)nkf)
+            return fail("counters out of range or inconsistent with the section counts");
+        if (!r.se3(L.pose)) return fail("truncated or non-finite pose");
+        if (!unitQuat(L.pose)) return fail("pose rotation is not a unit quaternion");
+        // keyframes: id, age, Twc [7], keypoints, covis, localmap
+        if ((uint64_t)nkf * 76 > r.left()) return fail("keyframe count exceeds the blob");
+        int prev = -1;
+        for (uint32_t k = 0; k < nkf; k++) {
+            int32_t id, age;
+            Se3 T;
+            if (!r.i32(id) || !r.i32(age) || !r.se3(T)) return fail("truncated or non-finite keyframe");
+            if (!unitQuat(T)) return fail("keyframe rotation is not a unit quaternion");
+            if (id <= prev || id >= L.n_kf_ids) return fail("keyframe ids not ascending, or not below n_kf_ids");
+            if (age < 0 || age > (1 << 30)) return fail("keyframe age out of range");
+            prev = id;
+            auto f = std::make_shared<Frame>();
+            f->init(&cam, cell);
+            f->id = -1 - age;   // the frame that saved the map is frame -1 of this session
+            f->kfid = id;
+            f->setTwc(T);
+            uint32_t nkp;
+            if (!r.count(nkp, 78)) return fail("keypoint count exceeds the blob");
+            int pk = -1;
+            for (uint32_t i = 0; i < nkp; i++) {
+                Keypoint p;
+                ok = r.i32(p.id) && r.f32(p.px) && r.f32(p.py) && r.f32(p.ux) && r.f32(p.uy);
+                for (int c = 0; c < 3; c++) ok = ok && r.f64(p.bv[c]);
+                ok = ok && r.flag(p.is3d) && r.flag(p.has_desc) && r.raw(p.desc, 32);
+                if (!ok) return fail("truncated, non-finite or non-boolean keypoint");
+                if (p.id <= pk || p.id >= L.n_mp_ids) return fail("keypoint ids not ascending, or not below n_mp_ids");
+                if (!(fabsf(p.px) <= 16777216.f && fabsf(p.py) <= 16777216.f)) return fail("keypoint position out of range");
+                pk = p.id;
+                f->add(p);
+            }
+            uint32_t nc;
+            if (!r.count(nc, 8)) return fail("covisibility count exceeds the blob");
+            int pc = -1;
+            for (uint32_t i = 0; i < nc; i++) {
+                int32_t kf, cnt;
+                if (!r.i32(kf) || !r.i32(cnt)) return fail("truncated covisibility");
+                if (kf <= pc) return fail("covisibility ids not ascending");
+                pc = kf;
+                f->covis.emplace(kf, cnt);
+            }
+            uint32_t nl;
+            if (!r.count(nl, 4)) return fail("local map count exceeds the blob");
+            int pl = -1;
+            for (uint32_t i = 0; i < nl; i++) {
+                int32_t m;
+                if (!r.i32(m)) return fail("truncated local map");
+                // a local map lists candidates and outlives the map points culled since (buildMatchProblem skips those): an
+                // entry must be an id the counter has issued, not necessarily a map point of the blob
+                if (m <= pl || m >= L.n_mp_ids) return fail("local map ids not ascending, or not below n_mp_ids");
+                pl = m;
+                f->localmap.insert(m);
+            }
+            L.kfs.push_back(f);
+        }
+        // map points: id, anchor, observed, is3d, invd, p [3], obs, (kfid, desc, descdist), has_desc, desc
+        if ((uint64_t)nmp * 83 > r.left()) return fail("map point count exceeds the blob");
+        L.mps.reserve(nmp);
+        prev = -1;
+        for (uint32_t k = 0; k < nmp; k++) {
+            MapPoint m;
+            ok = r.i32(m.id) && r.i32(m.kfid) && r.flag(m.observed) && r.flag(m.is3d) && r.f64(m.invd);
+            for (int c = 0; c < 3; c++) ok = ok && r.f64(m.p[c]);
+            if (!ok) return fail("truncated, non-finite or non-boolean map point");
+            if (m.id <= prev || m.id >= L.n_mp_ids) return fail("map point ids not ascending, or not below n_mp_ids");
+            prev = m.id;
+            uint32_t no;
+            if (!r.count(no, 4)) return fail("observation count exceeds the blob");
+            int po = -1;
+            for (uint32_t i = 0; i < no; i++) {
+                int32_t o;
+                if (!r.i32(o)) return fail("truncated observations");
+                if (o <= po) return fail("observations not ascending");
+                po = o;
+                m.obs.insert(m.obs.end(), o);
+            }
+            uint32_t nd;
+            if (!r.count(nd, 40)) return fail("descriptor count exceeds the blob");
+            int pd = -1;
+            for (uint32_t i = 0; i < nd; i++) {
+                int32_t kf;
+                Desc d;
+                float dist;
+                if (!r.i32(kf) || !r.raw(d.b, 32) || !r.f32(dist)) return fail("truncated or non-finite keyframe descriptor");
+                if (kf <= pd) return fail("keyframe descriptors not ascending");
+                pd = kf;
+                m.kfdesc.emplace(kf, d);
+                m.descdist.emplace(kf, dist);
+            }
+            if (!r.flag(m.has_desc) || !r.raw(m.desc.b, 32)) return fail("truncated map point descriptor");
+            if (!m.has_desc)
+                for (int i = 0; i < 32; i++) if (m.desc.b[i]) return fail("a descriptor on a map point without one");
+            L.mps.push_back(std::move(m));
+        }
+        if (r.left() != 0) return fail("bytes after the last map point");
+        // Every reference names an issued id (0 <= id < its counter): a record of the blob, or a keyframe or map point removed
+        // since.  A live map holds the latter once keyframes leave it (filterKeyframes, the 30-keyframe window): removeObs
+        // leaves the anchor of a point whose last observation went, localBA erases covisibility entries lazily, a culled
+        // point stays in local maps.  The state machine looks every such id up with find() and skips a missing record, so
+        // keeping them makes the loaded map the saved one.
+        auto kf_ok = [&](int id) { return id >= 0 && id < L.n_kf_ids; };
+        auto mp_ok = [&](int id) { return id >= 0 && id < L.n_mp_ids; };
+        for (auto& f : L.kfs) {
+            for (auto& kv : f->kps) if (kv.second.is3d && !mp_ok(kv.first)) return fail("a 3-D keypoint names no issued map point");
+            for (auto& kv : f->covis) if (!kf_ok(kv.first)) return fail("a covisibility entry names no issued keyframe");
+        }
+        for (auto& m : L.mps) {
+            if (!kf_ok(m.kfid)) return fail("a map point's anchor names no issued keyframe");
+            for (int o : m.obs) if (!kf_ok(o)) return fail("an observation names no issued keyframe");
+            for (auto& kv : m.kfdesc) if (!kf_ok(kv.first)) return fail("a keyframe descriptor names no issued keyframe");
+        }
+        return true;
+    }
 
     // ------------------------------------------------------------------ MapManager pieces
     void removeObsFromCurr(int id) {
@@ -1305,6 +1584,9 @@ private:
         lost = true;
         lost_frames = 1;
         n_lost++;
+        buildRelocTable();
+    }
+    void buildRelocTable() {
         RelocTable& t = reloc_table;
         t.clear();
         std::vector<int> ids;

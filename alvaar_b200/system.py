@@ -23,6 +23,8 @@ def _bind():
     L.alva_system_lens_drops.argtypes = [_vp]
     L.alva_system_set_preset.argtypes = [_vp, _i32]
     L.alva_system_set_relocalisation.argtypes = [_vp, _i32]
+    L.alva_system_save_map.argtypes = [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]
+    L.alva_system_load_map.argtypes = [_vp, C.c_char_p, C.c_size_t]
     L.alva_system_num_matched.argtypes = [_vp]
     L.alva_system_configure.argtypes = [_vp, _i32, _i32] + [_f64] * 8
     L.alva_system_find_camera_pose.argtypes = [_vp, _vp, _vp]
@@ -185,3 +187,36 @@ class System:
         rc = self.L.alva_system_set_relocalisation(self.h, int(max_lost_frames))
         if rc != 0:
             raise AlvaError(f"alva_system_set_relocalisation -> {rc}: {self.L.alva_last_error().decode()}")
+
+    def save_map(self):
+        """-> the map as bytes (a versioned, self-contained blob; the format is in include/alva_b200.h), to resume the session
+        in a new System or to start another stream in this one's map and coordinate frame.  Allowed once initialised, also
+        while lost; it changes nothing.  AlvaError before the initialisation."""
+        # one serialisation per call: a buffer with room for the last blob and a quarter more; only a map that outgrew it
+        # (ALVA_E_CAPACITY, which reports the length) is serialised a second time
+        cap = getattr(self, "_map_cap", 1 << 20)
+        n = C.c_size_t(0)
+        buf = C.create_string_buffer(cap)
+        rc = self.L.alva_system_save_map(self.h, buf, cap, C.byref(n))
+        if rc == -3:
+            cap = n.value
+            buf = C.create_string_buffer(cap)
+            rc = self.L.alva_system_save_map(self.h, buf, cap, C.byref(n))
+        if rc == 0:
+            self._map_cap = max(1 << 16, n.value + n.value // 4)
+        if rc != 0:
+            raise AlvaError(f"alva_system_save_map -> {rc}: {self.L.alva_last_error().decode()}")
+        return buf.raw[:n.value]
+
+    def load_map(self, data):
+        """Replace the map with a blob from save_map() and enter the lost state.  Needs set_relocalisation(n > 0), and a System
+        configured with the same camera, lens and preset cell size as the one that saved it.  The next frames return status 4
+        (LOST) with the saved pose until one relocalises into the map; tracking then resumes with status 1 in the saved
+        coordinate frame, and new keyframe and map point ids continue from the saved map's.  After n lost frames the map is
+        discarded (status 2), as after any loss.  The blob is checked whole before anything changes: AlvaError for a blob that
+        fails a check or relocalisation off, and the System is left as it was.  configure, reset(), set_preset(),
+        set_distortion() and set_fisheye() discard a loaded map like any other."""
+        data = bytes(data)
+        rc = self.L.alva_system_load_map(self.h, data, len(data))
+        if rc != 0:
+            raise AlvaError(f"alva_system_load_map -> {rc}: {self.L.alva_last_error().decode()}")

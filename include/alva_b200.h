@@ -514,6 +514,49 @@ int  alva_system_set_preset(alva_system*, int preset);
  * ALVA_E_INVALID for a null handle or a negative value. */
 #define ALVA_STATUS_LOST 4
 int  alva_system_set_relocalisation(alva_system*, int max_lost_frames);
+/* The map as a self-contained byte string, to resume a session in a new handle or to start another stream in this one's map and
+ * coordinate frame.
+ *
+ * alva_system_save_map writes the map into buf (cap bytes) and its length into *bytes.  buf = NULL only queries the length; a
+ * short buffer returns ALVA_E_CAPACITY with *bytes set.  It is allowed once the system is initialised, also while lost (else
+ * ALVA_E_STATE), and changes nothing.
+ *
+ * alva_system_load_map replaces the map with a blob's and enters the lost state: the next frames return ALVA_STATUS_LOST with
+ * the saved pose until one relocalises into the map (status 1; new keyframe and map point ids continue from the saved
+ * counters), and after max_lost_frames failures the map is discarded (status 2).  It needs relocalisation on
+ * (alva_system_set_relocalisation > 0), else ALVA_E_STATE.  The whole blob is checked before anything changes; a blob that
+ * fails a check returns ALVA_E_INVALID and leaves the system as it was: bad magic / version, a byte count other than `bytes`,
+ * a camera, lens or grid cell size other than the configured ones, truncated or trailing data, ids not strictly ascending,
+ * counters above 2^30 or not above every stored id, a reference to an id never issued, a non-finite number, a rotation that
+ * is not a unit quaternion (|q|^2 off 1 by more than 1e-9) or a flag other than 0 / 1.
+ * configure, reset, set_preset, set_distortion and set_fisheye discard a loaded map as they discard any map.
+ *
+ * Format, version 1: little-endian, fixed-width fields, no padding (i32 / u32 / u64 / f32 / f64, u8 flags 0 or 1).
+ *   header     "ALMP", u32 version = 1, u64 total bytes, u32 keyframe count, u32 map point count
+ *   camera     i32 w, h; f64 fx, fy, cx, cy; i32 lens (0 pinhole, 1 radial-tangential, 2 fisheye); f64 coefficients [4]
+ *   grid       i32 cell size of the preset
+ *   counters   i32 n_kf_ids, n_mp_ids (the next ids), n_kf (= the keyframe count)
+ *   pose       f64 t [3], q [4] (x y z w): the pose the lost frames report
+ *   keyframes, ascending id:
+ *              i32 id; i32 age (frames from the keyframe's frame to the saving frame); f64 Twc t [3], q [4];
+ *              u32 n, then n keypoints, ascending id: i32 id; f32 px, py, ux, uy; f64 bv [3]; u8 is3d, has_desc; u8 desc [32]
+ *              u32 n, then n covisibility pairs, ascending keyframe id: i32 keyframe id, i32 count
+ *              u32 n, then n local map point ids, ascending
+ *   map points, ascending id:
+ *              i32 id, anchor keyframe id; u8 observed, is3d; f64 inverse depth; f64 p [3]
+ *              u32 n, then n observing keyframe ids, ascending
+ *              u32 n, then n (i32 keyframe id, u8 desc [32], f32 descriptor distance sum), ascending keyframe id
+ *              u8 has_desc; u8 desc [32]
+ * References (3-D keypoints' map points, anchors, observations, keyframe descriptors, covisibility, local maps) name issued
+ * ids, 0 <= id < the counter: a record of the blob, or a keyframe or map point removed since.  A live map names removed ones
+ * once keyframes leave it (keyframe filtering, the 30-keyframe window); the tracker looks every id up and skips missing
+ * records, so they are kept and the loaded map equals the saved one.  Rebuilt on load, not stored: a
+ * keyframe's grid, cell counts and keypoint counts (from its keypoints, inserted in ascending id order, and the cell size); Tcw
+ * (the inverse of Twc); the current frame (empty, as a lost frame; its keyframe is the newest, n_kf_ids - 1).  `observed` is
+ * saved as the lost state holds it (cleared for the current frame's points).  Frame ids restart at 0 in the loading session:
+ * a keyframe's frame id becomes -1 - age.  Time stamps are not stored (the motion model restarts after a relocalisation). */
+int  alva_system_save_map(alva_system*, uint8_t* buf, size_t cap, size_t* bytes);
+int  alva_system_load_map(alva_system*, const uint8_t* buf, size_t bytes);
 int  alva_system_find_camera_pose(alva_system*, const uint8_t* rgba, float* pose16);
 /* the same with the frame's time stamp (milliseconds) supplied by the caller instead of read from the system clock
  * (system.cpp:114): deterministic replays, and hosts that deliver frames faster than real time (two frames inside one

@@ -15,6 +15,7 @@
 // configure with zeros, then call alva_system_set_distortion(handle, k1, k2, p1, p2) (alva_b200.h).
 #pragma once
 #include <cstdint>
+#include <vector>
 #include "alva_b200.h"
 
 class System {
@@ -37,6 +38,21 @@ public:
     // not in the reference's class: OpenCV's equidistant fisheye lens (k1..k4 on theta; enabled = 0: the pinhole), for
     // wide-angle cameras; resets the tracker and the map; 0 or an ALVA_E_* code
     int setFisheye(int enabled, double k1, double k2, double k3, double k4) { return alva_system_set_fisheye(h_, enabled, k1, k2, k3, k4); }
+    // not in the reference's class: the map as bytes (alva_system_save_map / alva_system_load_map, alva_b200.h).  saveMap
+    // replaces `out` with the blob; loadMap needs setRelocalisation > 0 and enters the lost state.  0 or an ALVA_E_* code
+    // (one serialisation when `out`'s capacity already holds the map, e.g. when it is reused from call to call)
+    int saveMap(std::vector<uint8_t>& out) {
+        size_t n = 0;
+        out.resize(out.capacity() > 65536 ? out.capacity() : 65536);
+        int e = alva_system_save_map(h_, out.data(), out.size(), &n);
+        if (e == ALVA_E_CAPACITY) {
+            out.resize(n);
+            e = alva_system_save_map(h_, out.data(), out.size(), &n);
+        }
+        out.resize(e == 0 ? n : 0);
+        return e;
+    }
+    int loadMap(const std::vector<uint8_t>& blob) { return alva_system_load_map(h_, blob.data(), blob.size()); }
 
     // ---- the reference's wasm32 signatures
     int findCameraPose(int imageRGBADataPtr, int posePtr) { return findCameraPose(ptr<const uint8_t>(imageRGBADataPtr), ptr<float>(posePtr)); }
