@@ -17,7 +17,7 @@
 // candidate order inside the warp, the second is a 64-bit atomicMin on (distance, reversed processing index).
 #include "alva_common.cuh"
 #include "../../include/alva_b200.h"
-#include "camera_model.h"
+#include "map_geom.cuh"
 #include <math.h>
 
 namespace {
@@ -55,42 +55,14 @@ struct MatchParams {
     double dist[4];   // k1 k2 p1 p2 (LENS_RADTAN) or k1 k2 k3 k4 (LENS_FISHEYE)
 };
 
-__device__ __forceinline__ void quat_R(const double* q, double* R) {
-    const double n = sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
-    const double x = q[0] / n, y = q[1] / n, z = q[2] / n, w = q[3] / n;
-    const double tx = 2 * x, ty = 2 * y, tz = 2 * z;
-    const double twx = tx * w, twy = ty * w, twz = tz * w, txx = tx * x, txy = ty * x, txz = tz * x, tyy = ty * y, tyz = tz * y, tzz = tz * z;
-    R[0] = 1 - (tyy + tzz); R[1] = txy - twz; R[2] = txz + twy;
-    R[3] = txy + twz; R[4] = 1 - (txx + tzz); R[5] = tyz - twx;
-    R[6] = txz - twy; R[7] = tyz + twx; R[8] = 1 - (txx + tyy);
-}
-__device__ __forceinline__ void world_to_cam(const double* Twc, const double* X, double* c) {
-    double R[9], ti[3];
-    quat_R(Twc + 3, R);
-#pragma unroll
-    for (int i = 0; i < 3; i++) ti[i] = -(R[i] * Twc[0] + R[3 + i] * Twc[1] + R[6 + i] * Twc[2]);
-#pragma unroll
-    for (int i = 0; i < 3; i++) c[i] = (R[i] * X[0] + R[3 + i] * X[1] + R[6 + i] * X[2]) + ti[i];
-}
-__device__ __forceinline__ void project(const MatchParams& P, const double* c, float* px) {
-    const double iz = 1. / c[2];
-    const double x = (double)(float)(c[0] * iz), y = (double)(float)(c[1] * iz);   // cv::Point3f(x, y, 1.0)
-    px[0] = (float)(x * P.fx + P.cx);
-    px[1] = (float)(y * P.fy + P.cy);
-}
-// LENS_NONE: the zero-distortion projection above; LENS_RADTAN / LENS_FISHEYE: the lens models of camera_model.h
-enum { LENS_NONE = 0, LENS_RADTAN = 1, LENS_FISHEYE = 2 };
+using alva_geom::world_to_cam;
+using alva_geom::LENS_NONE;
+using alva_geom::LENS_RADTAN;
+using alva_geom::LENS_FISHEYE;
 template <int LENS>
 __device__ __forceinline__ void project_cam(const MatchParams& P, const double* c, float* px) {
-    if constexpr (LENS == LENS_RADTAN) {
-        const double K4[4] = {P.fx, P.fy, P.cx, P.cy};
-        alva_cam::project_dist(K4, P.dist, c, px);
-    } else if constexpr (LENS == LENS_FISHEYE) {
-        const double K4[4] = {P.fx, P.fy, P.cx, P.cy};
-        alva_cam::project_dist_fisheye(K4, P.dist, c, px);
-    } else {
-        project(P, c, px);
-    }
+    const double K4[4] = {P.fx, P.fy, P.cx, P.cy};
+    alva_geom::project_cam<LENS>(K4, P.dist, c, px);
 }
 
 // one CTA: observed flags, the frame's grid (cell -> keypoints in insertion order), per-keypoint result keys

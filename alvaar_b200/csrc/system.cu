@@ -23,6 +23,8 @@
 //   ba_local     local bundle adjustment, both solves + flags     alva_k_ba_local                   (optimizer.cpp:251-359)
 //   relocalise   a lost frame against the frozen map              alva_k_hamming_knn2_grouped, match rules, alva_k_p3p_ransac, alva_k_pnp
 //                (not in the reference: alva_system_set_relocalisation)
+//   reacquire    fresh detections against the frozen map          alva_k_match_frame_to_map (reacquire.cu)
+//                (not in the reference: alva_system_set_localisation_only)
 // There is no CPU fallback: configure() fails without an sm_90 (H100) device.  Lens distortion: the JS shim always passes zeros
 // (system.js:84-141) and configure() rejects non-zero coefficients; setDistortion() (alva_system_set_distortion) sets them on a
 // configured System, and setFisheye() (alva_system_set_fisheye) selects OpenCV's equidistant fisheye model instead.  With a
@@ -217,6 +219,7 @@ struct CudaBackend {
         void** rbufs[] = {(void**)&reloc_quality_dev, (void**)&reloc_tab, (void**)&reloc_ws};
         for (void** b : rbufs) if (*b) { cudaFree(*b); *b = nullptr; }
         reloc_tab_bytes = 0; reloc_ws_cap = 0; reloc_loaded = false;
+        rq.release();
         has_dist = fisheye = false;
         cap = cap_alloc = 0;
         cell = 40;
@@ -536,20 +539,8 @@ struct CudaBackend {
         const int n_grp = (int)T.mp_id.size(), n_rows = (int)(T.desc.size() / 32);
         if (nq > cap) { alva_set_error("System: %d queries exceed the frame capacity %d", nq, cap); return ALVA_E_CAPACITY; }
         if (nq == 0 || n_grp == 0) return 0;
-        const size_t ds_b = al256((size_t)(n_grp + 1) * 4), w_b = al256((size_t)n_grp * 24), d_b = al256((size_t)n_rows * 32),
-                     k_b = al256((size_t)n_grp * 4);
-        if (!reloc_loaded || reloc_version != T.version) {
-            if (ds_b + w_b + d_b + k_b > reloc_tab_bytes) {
-                if (reloc_tab) { SYS_CUDA(cudaStreamSynchronize(st)); cudaFree(reloc_tab); reloc_tab = nullptr; reloc_tab_bytes = 0; }
-                SYS_CUDA(cudaMalloc(&reloc_tab, ds_b + w_b + d_b + k_b));
-                reloc_tab_bytes = ds_b + w_b + d_b + k_b;
-            }
-            SYS_CUDA(cudaMemcpyAsync(reloc_tab, T.desc_start.data(), (size_t)(n_grp + 1) * 4, cudaMemcpyHostToDevice, st));
-            SYS_CUDA(cudaMemcpyAsync(reloc_tab + ds_b, T.wpt.data(), (size_t)n_grp * 24, cudaMemcpyHostToDevice, st));
-            SYS_CUDA(cudaMemcpyAsync(reloc_tab + ds_b + w_b, T.desc.data(), (size_t)n_rows * 32, cudaMemcpyHostToDevice, st));
-            reloc_version = T.version;
-            reloc_loaded = true;
-        }
+        if (int e = upload_table(T)) return e;
+        const size_t ds_b = al256((size_t)(n_grp + 1) * 4), w_b = al256((size_t)n_grp * 24), d_b = al256((size_t)n_rows * 32);
         const int32_t* d_start = (const int32_t*)reloc_tab;
         const double* d_wpt = (const double*)(reloc_tab + ds_b);
         const uint8_t* d_desc = reloc_tab + ds_b + w_b;
@@ -605,6 +596,69 @@ struct CudaBackend {
         R.mg.assign(hmg, hmg + R.n_match);
         R.o1.assign(ho1, ho1 + R.n_match);
         R.o2.assign(ho2, ho2 + R.n_match);
+        return 0;
+    }
+
+    // The frozen map's table on the device (reloc_tab: desc_start, wpt, desc, a per-group key list): uploaded only when its
+    // version changes -- once per loss, and once for a whole localisation-only session.
+    int upload_table(const alva_sys::RelocTable& T) {
+        if (reloc_loaded && reloc_version == T.version) return 0;
+        cudaStream_t st = ctx->stream;
+        const int n_grp = (int)T.mp_id.size(), n_rows = (int)(T.desc.size() / 32);
+        const size_t ds_b = al256((size_t)(n_grp + 1) * 4), w_b = al256((size_t)n_grp * 24), d_b = al256((size_t)n_rows * 32),
+                     k_b = al256((size_t)n_grp * 4);
+        if (ds_b + w_b + d_b + k_b > reloc_tab_bytes) {
+            if (reloc_tab) { SYS_CUDA(cudaStreamSynchronize(st)); cudaFree(reloc_tab); reloc_tab = nullptr; reloc_tab_bytes = 0; }
+            SYS_CUDA(cudaMalloc(&reloc_tab, ds_b + w_b + d_b + k_b));
+            reloc_tab_bytes = ds_b + w_b + d_b + k_b;
+        }
+        SYS_CUDA(cudaMemcpyAsync(reloc_tab, T.desc_start.data(), (size_t)(n_grp + 1) * 4, cudaMemcpyHostToDevice, st));
+        if (n_grp) SYS_CUDA(cudaMemcpyAsync(reloc_tab + ds_b, T.wpt.data(), (size_t)n_grp * 24, cudaMemcpyHostToDevice, st));
+        if (n_rows) SYS_CUDA(cudaMemcpyAsync(reloc_tab + ds_b + w_b, T.desc.data(), (size_t)n_rows * 32, cudaMemcpyHostToDevice, st));
+        reloc_version = T.version;
+        reloc_loaded = true;
+        return 0;
+    }
+
+    // Re-acquisition of a tracked frame against the frozen map (alva_system_set_localisation_only): the table stays resident
+    // (upload_table); per call ONE upload of the pose, the queries and the skip mask, the three launches of
+    // alva_k_match_frame_to_map, ONE download of the rows and distances and ONE synchronisation.
+    Staging rq;
+    int reacquire(const alva_sys::RelocTable& T, const uint8_t* skip, const double* Twc7, const float* qpx, const uint8_t* qdesc,
+                  const uint8_t* qkept, int nq, float radius, int32_t* row, int32_t* dist) {
+        cudaStream_t st = ctx->stream;
+        const int n_grp = (int)T.mp_id.size();
+        for (int i = 0; i < nq; i++) { row[i] = -1; dist[i] = -1; }
+        if (nq == 0 || n_grp == 0) return 0;
+        if (int e = upload_table(T)) return e;
+        const size_t need = 56 + (size_t)nq * 57 + (size_t)n_grp + 8 * 256;
+        if (!rq.fits(need)) if (int e = rq.init(need + need / 2)) return e;
+        rq.reset();
+        double* hT;
+        float* hp;
+        uint8_t *hd, *hk, *hs;
+        int32_t *hr, *hdist;
+        double* dT = rq.take<double>(7, &hT);
+        float* dp = rq.take<float>((size_t)2 * nq, &hp);
+        uint8_t* dd = rq.take<uint8_t>((size_t)32 * nq, &hd);
+        uint8_t* dk = rq.take<uint8_t>(nq, &hk);
+        uint8_t* ds = rq.take<uint8_t>(n_grp, &hs);
+        const size_t up_end = rq.off;
+        int32_t* dr = rq.take<int32_t>(nq, &hr);
+        const size_t down_off = (uint8_t*)dr - rq.d;
+        int32_t* ddist = rq.take<int32_t>(nq, &hdist);
+        const size_t down_end = rq.off;
+        memcpy(hT, Twc7, 56); memcpy(hp, qpx, (size_t)nq * 8); memcpy(hd, qdesc, (size_t)nq * 32); memcpy(hk, qkept, nq); memcpy(hs, skip, n_grp);
+        SYS_CUDA(cudaMemcpyAsync(rq.d, rq.h, up_end, cudaMemcpyHostToDevice, st));
+        const size_t ds_b = al256((size_t)(n_grp + 1) * 4), w_b = al256((size_t)n_grp * 24);   // upload_table's layout
+        const int lens = fisheye ? 2 : (has_dist ? 1 : 0);
+        if (int e = alva_k_match_frame_to_map(ctx, w, h, cell, fx, fy, cx, cy, lens, D4, dT, n_grp, (const double*)(reloc_tab + ds_b),
+                                              (const int32_t*)reloc_tab, reloc_tab + ds_b + w_b, ds, nq, dp, dd, dk, radius, dr, ddist))
+            return e;
+        SYS_CUDA(cudaMemcpyAsync(rq.h + down_off, rq.d + down_off, down_end - down_off, cudaMemcpyDeviceToHost, st));
+        SYS_CUDA(cudaStreamSynchronize(st));
+        memcpy(row, hr, (size_t)nq * 4);
+        memcpy(dist, hdist, (size_t)nq * 4);
         return 0;
     }
 
@@ -879,7 +933,19 @@ public:
     int getPose(double* Twc7) { core_.cur.Twc.to7(Twc7); return 0; }
     int setRelocalisation(int max_lost_frames) {
         if (!configured_) { alva_set_error("System: not configured"); return ALVA_E_STATE; }
-        core_.setRelocalisation(max_lost_frames);
+        if (int e = core_.setRelocalisation(max_lost_frames)) { alva_set_error("alva_system_set_relocalisation: %s", core_.map_error); return e; }
+        return 0;
+    }
+    // localisation only (system_core.h setLocalisationOnly): the map is frozen; fresh detections are matched against the
+    // resident relocalisation table on the device (CudaBackend::reacquire)
+    int setLocalisationOnly(int enabled) {
+        if (!configured_) { alva_set_error("System: not configured"); return ALVA_E_STATE; }
+        if (int e = core_.setLocalisationOnly(enabled != 0)) { alva_set_error("alva_system_set_localisation_only: %s", core_.map_error); return e; }
+        return 0;
+    }
+    // {mode on, frames re-acquisition ran on, points it supplied, points of its last run}
+    int localisationStats(int32_t* out4) const {
+        out4[0] = core_.frozen ? 1 : 0; out4[1] = core_.n_reacq_runs; out4[2] = core_.n_reacq_points; out4[3] = core_.reacq_last_points;
         return 0;
     }
     // The map blob (system_core.h: saveMap / loadMap).  Nothing on the device holds the map itself: the relocalisation table
@@ -994,6 +1060,13 @@ extern "C" int alva_system_set_preset(alva_system* s, int preset) { AlvaDeviceGu
 extern "C" int alva_system_set_relocalisation(alva_system* s, int max_lost_frames) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
     if (!s || max_lost_frames < 0) { alva_set_error("alva_system_set_relocalisation: bad argument"); return ALVA_E_INVALID; }
     return s->sys.setRelocalisation(max_lost_frames);
+}
+extern "C" int alva_system_set_localisation_only(alva_system* s, int enabled) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
+    if (!s || (enabled != 0 && enabled != 1)) { alva_set_error("alva_system_set_localisation_only: bad argument"); return ALVA_E_INVALID; }
+    return s->sys.setLocalisationOnly(enabled);
+}
+extern "C" int alva_system_localisation_stats(alva_system* s, int32_t* out4) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
+    return (s && out4) ? s->sys.localisationStats(out4) : ALVA_E_INVALID;
 }
 extern "C" int alva_system_save_map(alva_system* s, uint8_t* buf, size_t cap, size_t* bytes) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
     if (!s || !bytes) { alva_set_error("alva_system_save_map: bad argument"); return ALVA_E_INVALID; }

@@ -477,6 +477,10 @@ template <class B> struct BackendHasUnpx<B, std::void_t<decltype(std::declval<B&
 template <class B, class = void> struct BackendHasReloc : std::false_type {};
 template <class B> struct BackendHasReloc<B, std::void_t<decltype(std::declval<B&>().detect_lost(std::declval<std::vector<float>&>()))>> : std::true_type {};
 
+// a Backend may match fresh detections against the frozen map (reacquire); without it the localisation-only mode is refused
+template <class B, class = void> struct BackendHasReacquire : std::false_type {};
+template <class B> struct BackendHasReacquire<B, std::void_t<decltype(&B::reacquire)>> : std::true_type {};
+
 // ------------------------------------------------------------------------------------------------ flat problems handed to a Backend
 struct BaProblem {   // the layout of alva_k_ba_local
     int nkf = 0, nlm = 0, nobs = 0;
@@ -581,6 +585,10 @@ struct MapReader {
 //                                                          (the tracker's is left as it was); unpx() as after detect()
 //   int relocalise(const RelocTable&, const uint8_t* qdesc, const double* qbv, const double* quv, int nq, const double* K4,
 //                  float fx, float fy, RelocResult&)       grouped Hamming 2-NN, match rules, P3P-RANSAC (512) and PnP (relocaliseFrame)
+//   int reacquire(const RelocTable&, const uint8_t* skip, const double* Twc7, const float* qpx, const uint8_t* qdesc,
+//                 const uint8_t* qkept, int nq, float radius, int32_t* row, int32_t* dist)
+//                                                          alva_k_match_frame_to_map: per query the matched table row or -1
+//                                                          (localisation-only mode, reacquireFrame)
 //   optional: const float* unpx()                          see BackendHasUnpx
 template <class Backend>
 class SystemCore {
@@ -597,8 +605,42 @@ public:
         reloc_max = 0;
     }
 
-    // relocalisation after a tracking loss (0 = off: the reference's reset on the fourth failed pose); kept by reset()
-    void setRelocalisation(int max_lost_frames) { reloc_max = max_lost_frames; }
+    // relocalisation after a tracking loss (0 = off: the reference's reset on the fourth failed pose); kept by reset().  The
+    // localisation-only mode needs it: turning it off then is refused (MAP_STATE).
+    int setRelocalisation(int max_lost_frames) {
+        if (frozen && max_lost_frames <= 0) { map_error = "the localisation-only mode needs relocalisation"; return MAP_STATE; }
+        reloc_max = max_lost_frames;
+        return 0;
+    }
+
+    // ------------------------------------------------------------------ localisation only (not in the reference)
+    // Track against a frozen map: no keyframe, no triangulation, no local BA, no keyframe removal; keyframes and map points
+    // never change except the per-frame `observed` flag, and no id counter moves.  Points KLT loses come back through
+    // reacquireFrame.  A loss runs the relocalisation as usual but never resets the map.  Enabling needs relocalisation on
+    // and a map (MAP_STATE otherwise); it drops the frame's 2-D keypoints (only a keyframe could triangulate them) and keeps
+    // the relocalisation table loadMap or the loss built, or builds it for a tracking session.  The table is then neither
+    // rebuilt nor re-versioned until the mode ends.  Disabling is always allowed: mapping resumes on the next keyframe
+    // decision, ids continue from the counters, and a frame still lost gets max_lost_frames frames from then on.
+    // configure, reset, setPreset, setDistortion and setFisheye end the mode; loadMap keeps it (the loaded map is frozen).
+    int setLocalisationOnly(bool on) {
+        if (!on) {
+            if (frozen && lost) lost_frames = 0;
+            frozen = false;
+            reacq_pending = false;
+            return 0;
+        }
+        if (reloc_max <= 0 || !BackendHasReloc<Backend>::value || !BackendHasReacquire<Backend>::value) {
+            map_error = "relocalisation is off";
+            return MAP_STATE;
+        }
+        if (!ready_for_init) { map_error = "no map: not initialised"; return MAP_STATE; }
+        if (frozen) return 0;
+        for (const Keypoint& k : cur.all2d()) removeObsFromCurr(k.id);
+        if (!lost) buildRelocTable();
+        frozen = true;
+        reacq_pending = true;
+        return 0;
+    }
 
     // The fields of the reference's preset table (state.hpp:9-17) the state machine reads: State(w, h, cell) and its
     // frameMaxNumKeypoints_ (state.cpp:3-12), the current Frame's grid (Frame(calibration, cell), frame.cpp:9-15), the keyframe
@@ -634,6 +676,8 @@ public:
         pose_failed = 0;
         lost = false; lost_frames = 0;
         reloc_table.clear();
+        frozen = reacq_pending = false;
+        reacq_nocc = 0;
         // VisualFrontend::reset leaves the motion model and p3pReq_ alone (visual_frontend.cpp:718-728); so does this
     }
 
@@ -708,7 +752,9 @@ public:
         if (!data) { map_error = "null buffer"; return MAP_INVALID; }
         LoadedMap L;
         if (!parseMap(data, bytes, L)) return MAP_INVALID;
+        const bool keep_frozen = frozen;   // the localisation-only mode survives a load: the loaded map is frozen
         reset();
+        frozen = keep_frozen;
         // fresh containers: bucket counts, and so the iteration order of what is inserted next, depend on the blob alone
         keyframes = std::unordered_map<int, std::shared_ptr<Frame>>();
         mappoints = std::unordered_map<int, MapPoint>();
@@ -861,6 +907,9 @@ public:
 
     // ---- state the facade reads
     int reloc_max = 0;               // frames a lost track may relocalise for (0: off)
+    bool frozen = false;             // localisation only (setLocalisationOnly)
+    // re-acquisition in that mode: frames it ran on and points it supplied since construction, and the last run's points
+    int n_reacq_runs = 0, n_reacq_points = 0, reacq_last_points = 0;
     bool lost = false;
     int lost_frames = 0;             // consecutive frames returned as lost
     RelocTable reloc_table;
@@ -887,6 +936,8 @@ private:
     Backend& B;
     MotionModel motion;
     bool p3p_req = false;
+    bool reacq_pending = false;      // re-acquire on the next tracked frame (after freezing or a relocalisation)
+    int reacq_nocc = 0;              // the frame's occupied cells right after the last re-acquisition
     int pose_failed = 0, err = 0;
 
     // ------------------------------------------------------------------ map blob parsing: nothing of the system is touched
@@ -1572,6 +1623,7 @@ private:
             if (pose_failed > 3) { reset_requested = true; return false; }
         }
         motion.update(cur.Twc, timestamp);
+        if (frozen) { reacquireFrame(); return false; }
         return checkNewKeyframeRequired();
     }
 
@@ -1584,7 +1636,7 @@ private:
         lost = true;
         lost_frames = 1;
         n_lost++;
-        buildRelocTable();
+        if (!frozen) buildRelocTable();   // a frozen map keeps its table (and its device copy)
     }
     void buildRelocTable() {
         RelocTable& t = reloc_table;
@@ -1655,6 +1707,7 @@ private:
         reloc_last_matches = R.n_match;
         reloc_last_inliers = ok ? n2 - nout2 : 0;
         if (!ok) {
+            if (frozen) { if (lost_frames < INT32_MAX) lost_frames++; return 4; }   // a frozen map is never reset
             if (++lost_frames > reloc_max) { reset(); return 2; }
             return 4;
         }
@@ -1676,8 +1729,75 @@ private:
         lost = false;
         lost_frames = 0;
         n_relocalised++;
+        if (frozen) { reacq_pending = true; return 1; }   // no keyframe; the next tracked frame re-acquires
         kf = checkNewKeyframeRequired();
         return 1;
+    }
+
+    // ------------------------------------------------------------------ re-acquisition (localisation only)
+    // A tracked frame of a frozen map gets map points back without a keyframe.  It runs when (a) it is the first tracked frame
+    // after freezing or after a relocalisation, (b) the frame's occupied cells fell below 0.85 x their count right after the
+    // last re-acquisition, or (c) the frame has fewer than 30 3-D keypoints.  Then: the grid detector in the cells the
+    // frame's keypoints leave empty (the tracker's adaptive quality, as at a keyframe), ORB on the raw image, the lens drops of
+    // createKeyframe, and Backend::reacquire against the frozen table with the frame's map points masked out (radius 2 px, 4
+    // px below 30 3-D keypoints, as matchToMap's maxProjPxDist).  Each matched detection joins the frame as a 3-D keypoint of
+    // its map point, in detector order, while the frame holds fewer than twice the grid's cell count (the bound the
+    // keyframe's pruning keeps otherwise); the rest are discarded.  This frame's pose is not re-solved: the points enter PnP
+    // on the next frame.
+    void reacquireFrame() {
+        if (!(reacq_pending || cur.nocc < 0.85 * reacq_nocc || cur.n3d < 30)) return;
+        reacq_pending = false;
+        n_reacq_runs++;
+        reacq_last_points = 0;
+        if (max_kps - cur.nocc > 0) {
+            const std::vector<Keypoint> kps = cur.all();
+            std::vector<float> pts(2 * kps.size() + 2);
+            for (size_t i = 0; i < kps.size(); i++) { pts[2 * i] = kps[i].px; pts[2 * i + 1] = kps[i].py; }
+            std::vector<float> fresh;
+            if ((err = B.detect(pts.data(), (int)kps.size(), fresh)) < 0) return;
+            err = 0;
+            const float* un = backendUnpx();
+            std::vector<float> fresh_un;
+            if (un) fresh_un.assign(un, un + fresh.size());
+            const int nn = (int)fresh.size() / 2;
+            if (nn > 0) {
+                std::vector<uint8_t> desc(32 * (size_t)nn), kept(nn);
+                if ((err = B.describe(fresh.data(), nn, desc.data(), kept.data())) < 0) return;
+                err = 0;
+                for (int i = 0; i < nn; i++)
+                    if (lensDrop(fresh[2 * i], fresh[2 * i + 1], un ? &fresh_un[2 * (size_t)i] : nullptr)) kept[i] = 0;
+                const std::vector<int32_t>& ids = reloc_table.mp_id;   // ascending
+                std::vector<uint8_t> skip(ids.size() + 1, 0);
+                for (auto& kv : cur.kps) {
+                    auto it = std::lower_bound(ids.begin(), ids.end(), kv.first);
+                    if (it != ids.end() && *it == kv.first) skip[it - ids.begin()] = 1;
+                }
+                double T7[7];
+                cur.Twc.to7(T7);
+                std::vector<int32_t> row(nn, -1), dist(nn, -1);
+                if constexpr (BackendHasReacquire<Backend>::value)   // (the mode is refused without it)
+                    if ((err = B.reacquire(reloc_table, skip.data(), T7, fresh.data(), desc.data(), kept.data(), nn, cur.n3d < 30 ? 4.0f : 2.0f,
+                                           row.data(), dist.data())) < 0)
+                        return;
+                err = 0;
+                for (int i = 0; i < nn && cur.n < 2 * max_kps; i++) {
+                    if (row[i] < 0 || row[i] >= (int)ids.size()) continue;
+                    auto mp = mappoints.find(ids[row[i]]);
+                    if (mp == mappoints.end()) continue;
+                    Keypoint k;
+                    cur.compute(fresh[2 * i], fresh[2 * i + 1], k, un ? &fresh_un[2 * (size_t)i] : nullptr);
+                    k.id = ids[row[i]];
+                    k.is3d = true;
+                    k.has_desc = true;
+                    memcpy(k.desc, &desc[32 * (size_t)i], 32);
+                    mp->second.observed = true;
+                    cur.add(k);
+                    reacq_last_points++;
+                }
+                n_reacq_points += reacq_last_points;
+            }
+        }
+        reacq_nocc = cur.nocc;
     }
 
     void kltTracking() {   // kltTrackingFromMotionPrior (kltUsePrior_ = true)

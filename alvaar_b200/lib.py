@@ -70,6 +70,8 @@ _OPTIONAL = {
     "alva_k_project_points": [_vp, _vp, _i32, _vp, _vp, _vp],
     "alva_k_match_to_map_fisheye": [_vp, _i32, _i32, _i32, C.c_double, C.c_double, C.c_double, C.c_double, _vp, _i32, _vp, _vp, _i32, _i32,
                                     _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, C.c_float, C.c_float, _vp, _vp, _vp, _vp],
+    "alva_k_match_frame_to_map": [_vp, _i32, _i32, _i32, C.c_double, C.c_double, C.c_double, C.c_double, _i32, _vp, _vp, _i32, _vp, _vp,
+                                  _vp, _vp, _i32, _vp, _vp, _vp, C.c_float, _vp, _vp],
     "alva_k_undistort_points_fisheye": [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp],
     "alva_k_project_points_fisheye": [_vp, _vp, _i32, _vp, _vp, _vp],
     "alva_k_p3p_lmeds": [_vp, _i32, _i32, _vp, _vp, _vp, _i32, C.c_float, C.c_float, C.c_float, C.c_uint32, _vp, _vp, _vp],
@@ -243,6 +245,17 @@ class Context:
             self._chk(self.L.alva_k_match_to_map(*args))
         else:
             self._chk(self.L.alva_k_match_to_map_dist(*args, _f64x4(dist)))
+
+    def match_frame_to_map(self, w, h, cell, K, Twc, wpt, desc_start, desc, q_px, q_desc, q_kept, q_row, q_dist, radius=2.0, skip=None,
+                           lens=0, coef=None):
+        """the frozen map's re-acquisition of fresh detections -- see alva_k_match_frame_to_map.  Device tensors: Twc [7] float64,
+        wpt [n][3] float64, desc_start [n + 1] int32, desc [rows][32] uint8, skip [n] uint8 or None, q_px [nq][2] float32,
+        q_desc [nq][32] uint8, q_kept [nq] uint8; out q_row / q_dist [nq] int32.  lens 0 pinhole, 1 radial-tangential, 2 fisheye
+        with coef = its four coefficients."""
+        self._chk(self.L.alva_k_match_frame_to_map(self.h, w, h, cell, K[0], K[1], K[2], K[3], lens, _f64x4(coef) if lens else None,
+                                                   _ptr(Twc), wpt.shape[0], _ptr(wpt), _ptr(desc_start), _ptr(desc), _ptr(skip),
+                                                   q_px.shape[0], _ptr(q_px), _ptr(q_desc), _ptr(q_kept), float(radius), _ptr(q_row),
+                                                   _ptr(q_dist)))
 
     def undistort_points(self, px, counts, nframes, cap, K, dist, unpx):
         """cv::undistortPoints(px, unpx, K, D, K) for px [nframes][cap][2] float32 (counts: int32 [nframes] device tensor or None

@@ -25,6 +25,8 @@ def _bind():
     L.alva_system_set_relocalisation.argtypes = [_vp, _i32]
     L.alva_system_save_map.argtypes = [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]
     L.alva_system_load_map.argtypes = [_vp, C.c_char_p, C.c_size_t]
+    L.alva_system_set_localisation_only.argtypes = [_vp, _i32]
+    L.alva_system_localisation_stats.argtypes = [_vp, _vp]
     L.alva_system_num_matched.argtypes = [_vp]
     L.alva_system_configure.argtypes = [_vp, _i32, _i32] + [_f64] * 8
     L.alva_system_find_camera_pose.argtypes = [_vp, _vp, _vp]
@@ -220,3 +222,25 @@ class System:
         rc = self.L.alva_system_load_map(self.h, data, len(data))
         if rc != 0:
             raise AlvaError(f"alva_system_load_map -> {rc}: {self.L.alva_last_error().decode()}")
+
+    def set_localisation_only(self, enabled=True):
+        """Track against the current map without ever changing it: a venue or site map built once, a map shared between
+        devices, AR content that must stay where it was placed.  With it on there is no keyframe, no triangulation, no local BA
+        and no keyframe removal; keyframes, map points and ids stay as they are.  Map points the tracker loses are matched back
+        from the map without a keyframe (re-acquisition, on the first tracked frame after freezing or after a relocalisation,
+        when the frame's occupied grid cells fall below 0.85 x their count after the last re-acquisition, or below 30 3-D
+        keypoints).  A loss relocalises as usual (status 4, then 1) and never resets the map.  Usual flow:
+        set_relocalisation(n), load_map(blob), set_localisation_only(True); a live, initialised session can also freeze its own
+        map.  enabled=False resumes mapping on the next keyframe decision.  load_map() and set_clahe() keep the mode;
+        configuring, reset(), set_preset(), set_distortion() and set_fisheye() end it with the map.  AlvaError (nothing
+        changed) when enabling with relocalisation off or before the initialisation; set_relocalisation(0) is refused while
+        it is on."""
+        rc = self.L.alva_system_set_localisation_only(self.h, 1 if enabled else 0)
+        if rc != 0:
+            raise AlvaError(f"alva_system_set_localisation_only -> {rc}: {self.L.alva_last_error().decode()}")
+
+    def localisation_stats(self):
+        """{"on", "runs": frames re-acquisition ran on, "points": map points it returned, "last": those of its last run}"""
+        o = np.zeros(4, np.int32)
+        self.L.alva_system_localisation_stats(self.h, o.ctypes.data_as(_vp))
+        return dict(zip(("on", "runs", "points", "last"), o.tolist()))

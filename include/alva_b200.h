@@ -316,6 +316,27 @@ int alva_k_match_to_map_fisheye(alva_ctx*, int w, int h, int cell, double fx, do
                                 const float* obs_px, const int32_t* desc_start, const uint8_t* desc, int n_local, const int32_t* local_mp,
                                 float max_proj_err, float dist_ratio, int32_t* kp_match, float* kp_dist, int32_t* n_match,
                                 const double* fisheye4);
+/* Projection-gated matching of a tracked frame's fresh detections against a frozen map table (the re-acquisition of
+ * alva_system_set_localisation_only; not in the reference).  The gates of Mapper::matchToMap (mapper.cpp:354-587) for queries
+ * without a map point of their own.  Device pointers except coef4 (HOST, required for lens 1 / 2):
+ *   camera w, h, fx, fy, cx, cy; lens 0 pinhole, 1 radial-tangential (k1 k2 p1 p2), 2 fisheye (k1..k4); cell: the grid cell
+ *   Twc [7] = [t, q(x,y,z,w)] of the frame
+ *   table (the relocalisation table's layout, ascending map point id): wpt [n_mp][3] FP64, CSR desc_start [n_mp + 1] ->
+ *   desc [rows][32] (16-byte aligned); skip [n_mp] (optional): 1 = leave the row out (map points the frame already tracks)
+ *   queries: q_px [nq][2] FP32 distorted pixels as the detector returns them, q_desc [nq][32] (16-byte aligned), q_kept [nq]
+ *   (0 = never a candidate: no ORB descriptor, or a lens drop); radius: candidate distance in px (2, or 4 below 30 3-D
+ *   keypoints).
+ * Per row: skip, c = Tcw X with c_z >= 0.1 and |c_z| / |c| >= cos(atan(max(w / 2fx, h / 2fy))), the lens projection inside
+ * the image; candidates: the kept queries within radius, found through every grid cell the radius disc touches (the
+ * reference's getSurroundingKeypoints scans only the projection's cell and its upper-left neighbours); distance: the minimum
+ * Hamming distance over the row's descriptors; best / second best with `<=` from 51.2 in ascending query order, the best
+ * rejected if a second exists and 0.9 * second < best.  Per query: the row with the smallest distance, the highest row among
+ * equal ones.  Out: q_row [nq] the matched row or -1, q_dist [nq] its distance or -1.  One-to-one and deterministic; the
+ * CPU restatement is oracle/reacquire_oracle.c.  Three launches, no synchronisation. */
+int alva_k_match_frame_to_map(alva_ctx*, int w, int h, int cell, double fx, double fy, double cx, double cy, int lens,
+                              const double* coef4, const double* Twc, int n_mp, const double* wpt, const int32_t* desc_start,
+                              const uint8_t* desc, const uint8_t* skip, int nq, const float* q_px, const uint8_t* q_desc,
+                              const uint8_t* q_kept, float radius, int32_t* q_row, int32_t* q_dist);
 
 /* Local bundle adjustment, batched over nprob independent problems of identical dimensions
  * (Optimizer::localBA, src/slam/src/optimizer.cpp:4-531, solved the way ceres::Solve does with the reference's
@@ -514,6 +535,25 @@ int  alva_system_set_preset(alva_system*, int preset);
  * ALVA_E_INVALID for a null handle or a negative value. */
 #define ALVA_STATUS_LOST 4
 int  alva_system_set_relocalisation(alva_system*, int max_lost_frames);
+/* Localisation only: track against the current map without ever changing it -- a venue or site map built once, a map shared
+ * between devices, AR content that must stay where it was placed.  enabled = 1 freezes the map: no keyframe, no
+ * triangulation, no local BA and no keyframe removal; keyframes, map points and the id counters stay as they are.  Map points
+ * the tracker loses come back without a keyframe: on the first tracked frame after freezing or after a relocalisation, when
+ * the frame's occupied grid cells fall below 0.85 x their count after the last re-acquisition, or when it has fewer than 30
+ * 3-D keypoints, the grid detector runs in the empty cells and its ORB-described points are matched against the whole map
+ * (alva_k_match_frame_to_map); matched points join the frame as 3-D keypoints and enter the pose on the next frame.  A loss
+ * relocalises as usual (status 4, then 1) but the map is never reset, whatever max_lost_frames says; statuses are 1 and 4, never
+ * 2.  The usual flow is set_relocalisation(n) -> load_map(blob) -> set_localisation_only(1); a live, initialised session can
+ * also freeze its own map (the frame's 2-D keypoints are dropped: only a keyframe could triangulate them).  enabled = 0
+ * resumes mapping on the next keyframe decision, with ids continuing from the counters; a frame still lost then gets
+ * max_lost_frames frames.  load_map and set_clahe keep the mode (a loaded map stays frozen); configure, reset, set_preset,
+ * set_distortion and set_fisheye discard the map and end it.  A refusal changes nothing: ALVA_E_INVALID for a null handle or
+ * enabled other than 0 / 1; ALVA_E_STATE before configure, or when enabling with relocalisation off or before the
+ * initialisation; alva_system_set_relocalisation(0) returns ALVA_E_STATE while the mode is on.  Disabling is always allowed. */
+int  alva_system_set_localisation_only(alva_system*, int enabled);
+/* out4 = {mode on, frames re-acquisition ran on, map points it returned to the frame, those of its last run}, since the
+ * handle was created */
+int  alva_system_localisation_stats(alva_system*, int32_t* out4);
 /* The map as a self-contained byte string, to resume a session in a new handle or to start another stream in this one's map and
  * coordinate frame.
  *

@@ -53,6 +53,9 @@ public:
         return e;
     }
     int loadMap(const std::vector<uint8_t>& blob) { return alva_system_load_map(h_, blob.data(), blob.size()); }
+    // not in the reference's class: track against the map without changing it (alva_system_set_localisation_only); needs
+    // setRelocalisation > 0 and a map (loaded or initialised); loadMap keeps it on.  0 or an ALVA_E_* code
+    int setLocalisationOnly(bool enabled) { return alva_system_set_localisation_only(h_, enabled ? 1 : 0); }
 
     // ---- the reference's wasm32 signatures
     int findCameraPose(int imageRGBADataPtr, int posePtr) { return findCameraPose(ptr<const uint8_t>(imageRGBADataPtr), ptr<float>(posePtr)); }
