@@ -36,6 +36,9 @@ struct alva_ctx {
     size_t knn_ws_bytes = 0;
     void* clahe_ws = nullptr;       // alva_k_clahe's per-tile LUTs [frames][tiles_y][tiles_x][256] (clahe.cu)
     size_t clahe_ws_bytes = 0;
+    // bumped whenever one of the workspace pointers above changes (a grown buffer frees the old one): a CUDA graph that
+    // baked in this context's workspaces is replayed only while the epoch it was captured at is current (pipeline.cu)
+    uint64_t ws_epoch = 0;
     // fork / join inside one entry point (BA: the structure kernels run beside the first linearisation).  Created with the
     // context so that nothing is allocated while a caller captures `stream` into a CUDA graph.
     cudaStream_t aux_stream = nullptr;
@@ -59,6 +62,7 @@ struct AlvaDeviceGuard {
 
 void alva_set_error(const char* fmt, ...);
 void* alva_scratch(alva_ctx* ctx, size_t bytes);   // device scratch, valid until the next call
+extern uint64_t alva_g_options_epoch;   // bumped whenever alva_set_option changes a value (ba.cu)
 bool alva_make_tmap(CUtensorMap* map, CUtensorMapDataType dt, int rank, const void* base,
                     const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box);
 

@@ -52,6 +52,7 @@ bool alva_make_tmap(CUtensorMap* map, CUtensorMapDataType dt, int rank, const vo
 
 void* alva_scratch(alva_ctx* ctx, size_t bytes) {
     if (bytes > ctx->scratch_bytes) {
+        ctx->ws_epoch++;
         if (ctx->scratch) {
             cudaStreamSynchronize(ctx->stream);
             cudaFree(ctx->scratch);

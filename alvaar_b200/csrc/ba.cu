@@ -1508,6 +1508,7 @@ static int ba_prepare(alva_ctx* ctx, int nprob, int nkf, int nlm, int nobs, cons
     const size_t per = align_up(ba_ws_bytes(nkf, nlm, nobs, nblk) + (local ? per_local : 0), 256);
     const size_t tab = align_up(sizeof(BaProblem) * nprob, 256);
     if (tab + per * nprob > ctx->ba_ws_bytes) {
+        ctx->ws_epoch++;
         if (ctx->ba_ws) { ALVA_CUDA(cudaStreamSynchronize(ctx->stream)); ALVA_CUDA(cudaFree(ctx->ba_ws)); ctx->ba_ws = nullptr; ctx->ba_ws_bytes = 0; }
         ALVA_CUDA(cudaMalloc(&ctx->ba_ws, tab + per * nprob));
         ctx->ba_ws_bytes = tab + per * nprob;
@@ -1758,20 +1759,26 @@ int alva_g_ba_overlap = 1;   // pipeline.cu: local BA on its own stream beside t
 extern int alva_g_frontend_antipodal, alva_g_frontend_variant, alva_g_frontend_prefetch, alva_g_frontend_ctas;   // frontend.cu
 extern int alva_g_knn_mma, alva_g_knn_mma_mode, alva_g_knn_mma_kind;
 extern int alva_g_pipeline_graphs, alva_g_ba_lag;   // pipeline.cu
+uint64_t alva_g_options_epoch = 0;
+// a change of value bumps the options epoch: alva_pipeline then re-captures graphs that may have baked in the old choice
+static int set_option(int& opt, int value) {
+    if (opt != value) { opt = value; alva_g_options_epoch++; }
+    return 0;
+}
 extern "C" int alva_set_option(const char* name, int value) {
-    if (name && !strcmp(name, "ba_dense_schur")) { g_ba_dense_schur = value ? 1 : 0; return 0; }
-    if (name && !strcmp(name, "ba_ctl_threads") && (value == 256 || value == 512 || value == 1024)) { g_ba_ctl_threads = value; return 0; }
-    if (name && !strcmp(name, "frontend_antipodal")) { alva_g_frontend_antipodal = value ? 1 : 0; return 0; }
-    if (name && !strcmp(name, "frontend_variant") && (value == 0 || value == 2)) { alva_g_frontend_variant = value; return 0; }
-    if (name && !strcmp(name, "frontend_ctas") && (value == 4 || value == 5)) { alva_g_frontend_ctas = value; return 0; }
-    if (name && !strcmp(name, "frontend_prefetch")) { alva_g_frontend_prefetch = value ? 1 : 0; return 0; }
-    if (name && !strcmp(name, "pipeline_graphs")) { alva_g_pipeline_graphs = value ? 1 : 0; return 0; }
-    if (name && !strcmp(name, "pipeline_ba_lag")) { alva_g_ba_lag = value ? 1 : 0; return 0; }
-    if (name && !strcmp(name, "pipeline_ba_overlap")) { alva_g_ba_overlap = value ? 1 : 0; return 0; }
-    if (name && !strcmp(name, "knn_qpw") && (value == 4 || value == 8)) { alva_g_knn_qpw = value; return 0; }
-    if (name && !strcmp(name, "knn_mma") && value >= 0 && value <= 2) { alva_g_knn_mma = value; return 0; }
-    if (name && !strcmp(name, "knn_mma_kind") && (value == 0 || value == 1)) { alva_g_knn_mma_kind = value; return 0; }
-    if (name && !strcmp(name, "knn_mma_mode") && value >= 0 && value <= 2) { alva_g_knn_mma_mode = value; return 0; }
+    if (name && !strcmp(name, "ba_dense_schur")) return set_option(g_ba_dense_schur, value ? 1 : 0);
+    if (name && !strcmp(name, "ba_ctl_threads") && (value == 256 || value == 512 || value == 1024)) return set_option(g_ba_ctl_threads, value);
+    if (name && !strcmp(name, "frontend_antipodal")) return set_option(alva_g_frontend_antipodal, value ? 1 : 0);
+    if (name && !strcmp(name, "frontend_variant") && (value == 0 || value == 2)) return set_option(alva_g_frontend_variant, value);
+    if (name && !strcmp(name, "frontend_ctas") && (value == 4 || value == 5)) return set_option(alva_g_frontend_ctas, value);
+    if (name && !strcmp(name, "frontend_prefetch")) return set_option(alva_g_frontend_prefetch, value ? 1 : 0);
+    if (name && !strcmp(name, "pipeline_graphs")) return set_option(alva_g_pipeline_graphs, value ? 1 : 0);
+    if (name && !strcmp(name, "pipeline_ba_lag")) return set_option(alva_g_ba_lag, value ? 1 : 0);
+    if (name && !strcmp(name, "pipeline_ba_overlap")) return set_option(alva_g_ba_overlap, value ? 1 : 0);
+    if (name && !strcmp(name, "knn_qpw") && (value == 4 || value == 8)) return set_option(alva_g_knn_qpw, value);
+    if (name && !strcmp(name, "knn_mma") && value >= 0 && value <= 2) return set_option(alva_g_knn_mma, value);
+    if (name && !strcmp(name, "knn_mma_kind") && (value == 0 || value == 1)) return set_option(alva_g_knn_mma_kind, value);
+    if (name && !strcmp(name, "knn_mma_mode") && value >= 0 && value <= 2) return set_option(alva_g_knn_mma_mode, value);
     alva_set_error("alva_set_option: unknown option");
     return ALVA_E_INVALID;
 }

@@ -179,6 +179,7 @@ extern "C" int alva_k_clahe(alva_ctx* ctx, const uint8_t* src, uint8_t* dst, int
     }
     const size_t bytes = (size_t)nframes * tiles_x * tiles_y * 256;
     if (bytes > ctx->clahe_ws_bytes) {
+        ctx->ws_epoch++;
         if (ctx->clahe_ws) {
             ALVA_CUDA(cudaStreamSynchronize(ctx->stream));
             cudaFree(ctx->clahe_ws);

@@ -503,6 +503,7 @@ extern "C" int alva_k_detect_grid(alva_ctx* ctx, const uint8_t* gray, int w, int
     const size_t cand_b = (size_t)nframes * ncells * sizeof(float4);
     const size_t need = occ_b + hmap_b + mask_b + cand_b + 1024;
     if (need > ctx->det_ws_bytes) {
+        ctx->ws_epoch++;
         if (ctx->det_ws) { ALVA_CUDA(cudaStreamSynchronize(ctx->stream)); ALVA_CUDA(cudaFree(ctx->det_ws)); ctx->det_ws = nullptr; ctx->det_ws_bytes = 0; }
         ALVA_CUDA(cudaMalloc(&ctx->det_ws, need));
         ctx->det_ws_bytes = need;

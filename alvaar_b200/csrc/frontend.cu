@@ -1252,6 +1252,7 @@ extern "C" int alva_h_frontend(alva_ctx* ctx, const uint8_t* rgba_host, int w, i
     const size_t cnt_bytes = ((size_t)nframes * sizeof(int32_t) + 255) & ~(size_t)255;
     const size_t need = in_bytes + key_bytes + cnt_bytes + 512;
     if (need > ctx->dev_stage_bytes) {
+        ctx->ws_epoch++;
         if (ctx->dev_stage) { ALVA_CUDA(cudaStreamSynchronize(ctx->stream)); ALVA_CUDA(cudaFree(ctx->dev_stage)); ctx->dev_stage = nullptr; }
         ALVA_CUDA(cudaMalloc(&ctx->dev_stage, need));
         ctx->dev_stage_bytes = need;

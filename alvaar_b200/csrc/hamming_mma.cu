@@ -404,6 +404,7 @@ int alva_knn2_mma_launch(alva_ctx* ctx, const uint8_t* q, int nq, const uint8_t*
     const size_t a_bytes = (size_t)a_tiles * BLOB, b_bytes = (size_t)b_tiles * BLOB;
     const size_t need = off_bytes + map_bytes + a_bytes + b_bytes;
     if (need > ctx->knn_ws_bytes) {
+        ctx->ws_epoch++;
         if (ctx->knn_ws) { ALVA_CUDA(cudaStreamSynchronize(ctx->stream)); ALVA_CUDA(cudaFree(ctx->knn_ws)); ctx->knn_ws = nullptr; ctx->knn_ws_bytes = 0; }
         ALVA_CUDA(cudaMalloc(&ctx->knn_ws, need + need / 8));
         ctx->knn_ws_bytes = need + need / 8;

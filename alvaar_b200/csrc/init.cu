@@ -267,6 +267,7 @@ extern "C" int alva_k_essential_5pt(alva_ctx* ctx, int nprob, int cap, const dou
     if (!ctx->init_tab || ctx->init_tab_len != P.table_len || ctx->init_tab_seed != seed) {
         std::vector<int32_t> host_tab;
         make_rnd_table_init(seed, P.table_len, host_tab);
+        ctx->ws_epoch++;
         if (ctx->init_tab) { ALVA_CUDA(cudaStreamSynchronize(ctx->stream)); ALVA_CUDA(cudaFree(ctx->init_tab)); ctx->init_tab = nullptr; }
         ALVA_CUDA(cudaMalloc(&ctx->init_tab, (size_t)P.table_len * 4));
         ALVA_CUDA(cudaMemcpy(ctx->init_tab, host_tab.data(), (size_t)P.table_len * 4, cudaMemcpyHostToDevice));

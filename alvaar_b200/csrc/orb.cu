@@ -483,6 +483,7 @@ extern "C" int alva_k_orb_detect(alva_ctx* ctx, const uint8_t* gray, int w, int 
     const size_t b_pts2 = al((size_t)nframes * out_cap * 8), b_ang = al((size_t)nframes * out_cap * 4), b_kept = al((size_t)nframes * out_cap);
     const size_t need = 2 * b_keys + b_pts + b_resp + 2 * b_cnt + b_img + b_pts2 + b_ang + b_kept;
     if (need > ctx->det_ws_bytes) {
+        ctx->ws_epoch++;
         if (ctx->det_ws) { ALVA_CUDA(cudaStreamSynchronize(ctx->stream)); ALVA_CUDA(cudaFree(ctx->det_ws)); ctx->det_ws = nullptr; ctx->det_ws_bytes = 0; }
         ALVA_CUDA(cudaMalloc(&ctx->det_ws, need));
         ctx->det_ws_bytes = need;

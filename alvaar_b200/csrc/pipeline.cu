@@ -97,16 +97,30 @@ struct alva_pipeline {
     long long step_index = 0;
     std::vector<void*> allocs;
     // CUDA graphs: the per-frame stages of a frame range (keyed by input pointer and range: the kernel arguments are baked in) and
-    // the step's local-BA chain are each captured once, after a first direct run has sized every scratch buffer, and replayed
-    // with one launch (~60 + ~50 dependent launches per step otherwise).  Not used while profiling: a graph cannot carry the
-    // per-launch event pairs alva_pipeline_frontend_ms reads.
-    struct Graph { cudaGraphExec_t exec = nullptr; long long launches = 0; };
+    // the step's local-BA chain are each captured after a first direct run has sized every scratch buffer, and replayed with one
+    // launch (~60 + ~50 dependent launches per step otherwise).  A graph also bakes in the workspaces of the contexts its kernels
+    // run on (ctx / sel_ctx for a frame range, ba_ctx[k] for BA slot k) and the kernel variants the options chose.  Any call on
+    // those contexts may grow a workspace and free the old one, and alva_set_option may pick another kernel, so a graph records
+    // the contexts' workspace epochs and the options epoch it was captured under and is replayed only while they are current;
+    // otherwise it is dropped, the key runs directly again and is captured anew on its next use (a capture thus always follows
+    // a direct run under the same workspaces and options, and never has to grow a buffer, which would synchronise the stream
+    // and end the capture).  Not used while profiling: a graph cannot carry the per-launch event pairs alva_pipeline_frontend_ms
+    // reads.
+    struct Epochs {
+        uint64_t ws0 = 0, ws1 = 0, opt = 0;
+        bool operator==(const Epochs& o) const { return ws0 == o.ws0 && ws1 == o.ws1 && opt == o.opt; }
+    };
+    struct Graph {
+        cudaGraphExec_t exec = nullptr;
+        long long launches = 0;
+        int runs = 0;     // direct runs under `seen` (capture after the first)
+        Epochs seen;      // epochs after the last direct run or capture
+    };
     std::map<std::tuple<const uint8_t*, int, int>, Graph> frame_graphs;
-    std::map<std::tuple<const uint8_t*, int, int>, int> frame_runs;   // direct runs seen per key (capture after the first)
     Graph ba_graph[NBA];
-    int ba_runs[NBA] = {0, 0, 0};
     bool graphs_failed = false;
     long long graph_replays = 0;
+    long long graphs_captured = 0;   // cumulative: a re-capture after a workspace or option change counts again
 };
 
 static int palloc(alva_pipeline* p, void** ptr, size_t bytes) {
@@ -392,7 +406,24 @@ static bool capture_graph(alva_pipeline* p, cudaStream_t st, alva_pipeline::Grap
     if (g) cudaGraphDestroy(g);
     if (!ok) { cudaGetLastError(); out.exec = nullptr; return false; }
     out.launches = n;
+    p->graphs_captured++;
     return true;
+}
+
+static alva_pipeline::Epochs epochs_now(const alva_ctx* a, const alva_ctx* b) {
+    alva_pipeline::Epochs e;
+    e.ws0 = a->ws_epoch;
+    e.ws1 = b ? b->ws_epoch : 0;
+    e.opt = alva_g_options_epoch;
+    return e;
+}
+
+// drop a graph (and the direct runs it would be captured after) if a workspace or option it depends on changed since
+static void graph_validate(alva_pipeline::Graph& g, const alva_pipeline::Epochs& now) {
+    if (g.seen == now) return;
+    if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }   // a launch still in flight completes first
+    g.runs = 0;
+    g.seen = now;
 }
 
 // the BA chain itself, on slot k's stream (pristine copies -> working copies, then the solve)
@@ -416,18 +447,21 @@ static int pipeline_ba_launch(alva_pipeline* p, int k) {
     ALVA_CUDA(cudaStreamWaitEvent(st, p->ba_fork[k], 0));
     p->ba_forked[k] = true;
     p->ba_last = k;
-    if (graphs_on(p)) {
-        if (!p->ba_graph[k].exec && p->ba_runs[k] >= 1 && !capture_graph(p, st, p->ba_graph[k], [&] { return pipeline_ba_body(p, k); }))
-            p->graphs_failed = true;
-        if (p->ba_graph[k].exec) {
-            ALVA_CUDA(cudaGraphLaunch(p->ba_graph[k].exec, st));
-            p->ctx->launches += p->ba_graph[k].launches;
-            p->graph_replays++;
-            return 0;
-        }
+    if (!graphs_on(p)) return pipeline_ba_body(p, k);
+    alva_pipeline::Graph& g = p->ba_graph[k];
+    graph_validate(g, epochs_now(p->ba_ctx[k], nullptr));
+    if (!g.exec && g.runs >= 1 && !capture_graph(p, st, g, [&] { return pipeline_ba_body(p, k); }))
+        p->graphs_failed = true;
+    if (g.exec) {
+        ALVA_CUDA(cudaGraphLaunch(g.exec, st));
+        p->ctx->launches += g.launches;
+        p->graph_replays++;
+        return 0;
     }
-    p->ba_runs[k]++;
-    return pipeline_ba_body(p, k);
+    g.runs++;
+    const int e = pipeline_ba_body(p, k);
+    g.seen = epochs_now(p->ba_ctx[k], nullptr);   // what the run grew is what a capture will bake in
+    return e;
 }
 
 // main stream waits for slot k's chain; a lagged slot's results go to the public buffers
@@ -492,14 +526,15 @@ static int pipeline_ready(alva_pipeline* p) {
     return 0;
 }
 
-// the per-frame stages of frames [f0, f0 + nf): a graph replay when one exists for this (input, range), else direct launches
-// (the first direct run of a key sizes the scratch buffers; the second call captures)
+// the per-frame stages of frames [f0, f0 + nf): a graph replay when one exists for this (input, range) and the workspaces and
+// options it baked in are current, else direct launches (the first direct run of a key sizes the scratch buffers; the next
+// call captures)
 static int pipeline_frames_auto(alva_pipeline* p, const uint8_t* rgba_dev, int f0, int nf, bool timed, bool fork_ba) {
     if (!graphs_on(p)) return pipeline_frames(p, rgba_dev, f0, nf, timed, fork_ba);
     if (fork_ba) if (int e = pipeline_ba_fork(p)) return e;   // the BA chain is its own graph on its own stream
-    const auto key = std::make_tuple(rgba_dev, f0, nf);
-    alva_pipeline::Graph& g = p->frame_graphs[key];
-    if (!g.exec && p->frame_runs[key] >= 1 &&
+    alva_pipeline::Graph& g = p->frame_graphs[std::make_tuple(rgba_dev, f0, nf)];
+    graph_validate(g, epochs_now(p->ctx, p->sel_ctx));
+    if (!g.exec && g.runs >= 1 &&
         !capture_graph(p, p->ctx->stream, g, [&] { return pipeline_frames(p, rgba_dev, f0, nf, false, false); }))
         p->graphs_failed = true;
     if (g.exec) {
@@ -508,8 +543,10 @@ static int pipeline_frames_auto(alva_pipeline* p, const uint8_t* rgba_dev, int f
         p->graph_replays++;
         return 0;
     }
-    p->frame_runs[key]++;
-    return pipeline_frames(p, rgba_dev, f0, nf, timed, false);
+    g.runs++;
+    const int e = pipeline_frames(p, rgba_dev, f0, nf, timed, false);
+    g.seen = epochs_now(p->ctx, p->sel_ctx);
+    return e;
 }
 
 extern "C" int alva_pipeline_step_dev(alva_pipeline* p, const uint8_t* rgba_dev) { AlvaDeviceGuard guard__(p ? p->ctx : nullptr);
@@ -519,13 +556,11 @@ extern "C" int alva_pipeline_step_dev(alva_pipeline* p, const uint8_t* rgba_dev)
     return pipeline_ba_join(p);
 }
 
-// {graphs captured, graph launches so far, 1 if a capture failed and the pipeline fell back to direct launches}
+// {graphs captured so far (re-captures included), graph launches so far, 1 if a capture failed and the pipeline fell back to
+// direct launches}
 extern "C" int alva_pipeline_graph_stats(alva_pipeline* p, int32_t* out3) {
     if (!p || !out3) return ALVA_E_INVALID;
-    int n = 0;
-    for (int k = 0; k < alva_pipeline::NBA; k++) n += p->ba_graph[k].exec ? 1 : 0;
-    for (auto& kv : p->frame_graphs) n += kv.second.exec ? 1 : 0;
-    out3[0] = n; out3[1] = (int32_t)p->graph_replays; out3[2] = p->graphs_failed ? 1 : 0;
+    out3[0] = (int32_t)p->graphs_captured; out3[1] = (int32_t)p->graph_replays; out3[2] = p->graphs_failed ? 1 : 0;
     return 0;
 }
 

@@ -847,6 +847,7 @@ static int p3p_rnd_table(alva_ctx* ctx, uint32_t seed, int len) {
     if (ctx->p3p_tab && ctx->p3p_tab_len >= len && ctx->p3p_tab_seed == seed) return 0;
     std::vector<int32_t> host_tab;
     make_rnd_table(seed, len, host_tab);
+    ctx->ws_epoch++;
     if (ctx->p3p_tab) { ALVA_CUDA(cudaStreamSynchronize(ctx->stream)); ALVA_CUDA(cudaFree(ctx->p3p_tab)); ctx->p3p_tab = nullptr; }
     ALVA_CUDA(cudaMalloc(&ctx->p3p_tab, (size_t)len * 4));
     ALVA_CUDA(cudaMemcpy(ctx->p3p_tab, host_tab.data(), (size_t)len * 4, cudaMemcpyHostToDevice));

@@ -91,7 +91,8 @@ class Pipeline:
         self._chk(self.L.alva_pipeline_drain(self.h))
 
     def graph_stats(self):
-        """(CUDA graphs captured, graph launches so far, capture failed -> direct launches)"""
+        """(CUDA graphs captured so far, re-captures after a workspace or option change included; graph launches so far;
+        capture failed -> direct launches)"""
         out = (C.c_int32 * 3)()
         self.L.alva_pipeline_graph_stats.argtypes = [C.c_void_p, C.c_void_p]
         self._chk(self.L.alva_pipeline_graph_stats(self.h, out))

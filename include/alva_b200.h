@@ -388,6 +388,8 @@ int alva_k_ba_local(alva_ctx*, int nprob, int nkf, int nlm, int nobs, const doub
  * "ba_ctl_threads" = 256 | 512 | 1024: CTA size of the BA control kernels (default 1024; results differ at rounding level: the
  * block reductions partition differently).
  * "pipeline_graphs" = 0: alva_pipeline launches kernel by kernel instead of replaying CUDA graphs (default 1; results identical).
+ * Setting any option to a new value makes alva_pipeline capture its graphs again, so the kernels an option selects take
+ * effect at the next step (see alva_pipeline_graph_stats).
  * "knn_qpw" = 4 | 8: queries a warp of the Hamming matcher keeps in registers (8: 128 registers / 16 warps per SM;
  * 4: 80 registers / 24 warps per SM).  Results are identical.
  * "knn_mma" = 0 | 1 | 2: the tensor-core formulation of the Hamming matcher (hamming_mma.cu: descriptors expanded to +-1
@@ -462,7 +464,11 @@ int  alva_pipeline_wait(alva_pipeline*);
 int  alva_pipeline_profile(alva_pipeline*, int enable);
 int  alva_pipeline_frontend_ms(alva_pipeline*, float* ms, int n);   /* CUDA-event durations of the fused front-end launch */
 int  alva_pipeline_info(const alva_pipeline*, int32_t* out4);
-/* {CUDA graphs captured so far, graph launches so far, 1 if a capture failed and the pipeline fell back to direct launches} */
+/* {CUDA graphs captured so far, graph launches so far, 1 if a capture failed and the pipeline fell back to direct launches}.
+ * A graph is replayed only while the context workspaces it baked in and the alva_set_option values are those it was captured
+ * under; after a change (a call on the pipeline's context that grew a workspace, another pipeline on that context, an option
+ * set to a new value) it is dropped, its frame range runs directly once and is captured again -- the first count includes
+ * such re-captures. */
 int  alva_pipeline_graph_stats(alva_pipeline*, int32_t* out3);
 /* With alva_set_option("pipeline_ba_lag", 1) a step's local-BA chain is joined at the end of the NEXT step (two chains in
  * flight on two streams; a step then delivers the BA poses / summary of the step before it, as the reference's mapper thread
