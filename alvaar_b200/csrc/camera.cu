@@ -5,6 +5,9 @@
 //   alva_k_project_points    CameraCalibration::projectCamToImageDist (camera_calibration.cpp:34-55)
 //   alva_k_undistort_points_fisheye / alva_k_project_points_fisheye   the same two calls through OpenCV's equidistant fisheye
 //                            model (cv::fisheye::undistortPoints / projectPoints) instead of the radial-tangential one
+//   alva_k_rotate_priors     System's gyro mode (not in the reference): the KLT prior of a previous-frame keypoint turned by
+//                            the gyroscope's rotation and projected through the lens (alva_cam::rotate_prior), per lens
+//                            template
 // The arithmetic is camera_model.h, shared with the host state machine; this file is compiled with -fmad=false, so every
 // result is bit-identical to the host's and to OpenCV's (tests/test_gpu_distortion.py, tests/test_gpu_fisheye.py).
 #include "alva_common.cuh"
@@ -40,6 +43,24 @@ __global__ void __launch_bounds__(256) project_points_kernel(const double* __res
     if constexpr (FISH) alva_cam::project_dist_fisheye(c.K, c.D, p, o);
     else alva_cam::project_dist(c.K, c.D, p, o);
     uv[i] = make_float2(o[0], o[1]);
+}
+
+// System's gyro mode: the rotation-compensated KLT prior of every flagged point (alva_cam::rotate_prior); an unflagged point,
+// or one whose rotated ray is behind the camera or projects outside the image, keeps the prior it has
+struct RotArgs { double R[9]; };
+template <int LENS>
+__global__ void __launch_bounds__(256) rotate_priors_kernel(const double* __restrict__ bv, const uint8_t* __restrict__ flag, int n, int w,
+                                                            int h, const CamArgs c, const RotArgs r, float2* __restrict__ prior,
+                                                            uint8_t* __restrict__ rotated) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint8_t done = 0;
+    if (flag[i]) {
+        const double b[3] = {bv[3 * (size_t)i], bv[3 * (size_t)i + 1], bv[3 * (size_t)i + 2]};
+        float o[2];
+        if (alva_cam::rotate_prior(LENS, c.K, c.D, w, h, r.R, b, o)) { prior[i] = make_float2(o[0], o[1]); done = 1; }
+    }
+    rotated[i] = done;
 }
 
 bool cam_args(const char* fn, const double* K4, const double* D4, CamArgs& c) {
@@ -87,7 +108,44 @@ int project_checked(const char* fn, alva_ctx* ctx, const double* Xc, int n, cons
     return 0;
 }
 
+int rotate_launch(alva_ctx* ctx, const double* bv, const uint8_t* flag, int n, int w, int h, const double* K4, const double* D4, int lens,
+                  const double* R9, float* prior, uint8_t* rotated) {
+    if (n < 1) return 0;
+    CamArgs c;
+    RotArgs r;
+    for (int i = 0; i < 4; i++) { c.K[i] = K4[i]; c.D[i] = D4 ? D4[i] : 0.0; }
+    for (int i = 0; i < 9; i++) r.R[i] = R9[i];
+    const unsigned grid = (unsigned)((n + 255) / 256);
+    float2* p = (float2*)prior;
+    if (lens == 2) rotate_priors_kernel<2><<<grid, 256, 0, ctx->stream>>>(bv, flag, n, w, h, c, r, p, rotated);
+    else if (lens == 1) rotate_priors_kernel<1><<<grid, 256, 0, ctx->stream>>>(bv, flag, n, w, h, c, r, p, rotated);
+    else rotate_priors_kernel<0><<<grid, 256, 0, ctx->stream>>>(bv, flag, n, w, h, c, r, p, rotated);
+    ALVA_LAUNCH_CHECK(ctx);
+    return 0;
+}
+
 }  // namespace
+
+// System's gyro mode (system.cu, CudaBackend::klt_rotated): the coefficients are already checked, no argument checks
+int alva_rotate_priors_launch(alva_ctx* ctx, const double* bv, const uint8_t* flag, int n, int w, int h, const double* K4, const double* D4,
+                              int lens, const double* R9, float* prior, uint8_t* rotated) {
+    return rotate_launch(ctx, bv, flag, n, w, h, K4, D4, lens, R9, prior, rotated);
+}
+
+extern "C" int alva_k_rotate_priors(alva_ctx* ctx, const double* bv, const uint8_t* flag, int n, int w, int h, const double* K4,
+                                    const double* D4, int lens, const double* R9, float* prior, uint8_t* rotated) { AlvaDeviceGuard guard__(ctx);
+    const char* fn = "alva_k_rotate_priors";
+    if (!ctx || n < 0 || w < 1 || h < 1 || lens < 0 || lens > 2 || !R9 || (n > 0 && (!bv || !flag || !prior || !rotated))) {
+        alva_set_error("%s: bad argument", fn);
+        return ALVA_E_INVALID;
+    }
+    const double zero[4] = {0, 0, 0, 0};
+    CamArgs c;
+    if (!cam_args(fn, K4, D4 ? D4 : zero, c)) return ALVA_E_INVALID;
+    for (int i = 0; i < 9; i++) if (!isfinite(R9[i])) { alva_set_error("%s: non-finite rotation", fn); return ALVA_E_INVALID; }
+    if (((uintptr_t)prior) & 7) { alva_set_error("%s: prior must be 8-byte aligned", fn); return ALVA_E_INVALID; }
+    return rotate_launch(ctx, bv, flag, n, w, h, c.K, c.D, lens, R9, prior, rotated);
+}
 
 // host-side launches for callers that already hold the coefficients by value (system.cu): no argument checks
 int alva_undistort_points_launch(alva_ctx* ctx, const float* px, const int32_t* counts, int nframes, int cap, const double* K4,

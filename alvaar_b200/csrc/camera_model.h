@@ -267,4 +267,33 @@ ALVA_CAM_FN void project_dist_fisheye(const double* K4, const double* D4, const 
     out[1] = (float)(xd1_1 * f1 + c1);
 }
 
+// the pinhole branch of CameraCalibration::projectCamToImageDist as the state machine's Camera takes it: the normalised point
+// rounded to float, then scaled by K
+ALVA_CAM_FN void project_pinhole(const double* K4, const double* p, float* out) {
+    const double iz = 1. / p[2];
+    const double x = (double)(float)(p[0] * iz), y = (double)(float)(p[1] * iz);
+    out[0] = (float)(x * K4[0] + K4[2]);
+    out[1] = (float)(y * K4[1] + K4[3]);
+}
+
+// A rotation-compensated KLT prior (System's gyro mode, not in the reference): the bearing bv of a previous-frame keypoint
+// turned into the current camera, c = R^T bv (R = the camera's rotation from the previous frame to the current one, row-major),
+// and projected through the lens (0 pinhole, 1 radial-tangential, 2 fisheye; D4 unused for the pinhole) -- the infinite
+// homography, exact for a pure rotation.  Returns true and writes out[2] only when the ray is in front of the camera (z > 0)
+// and its projection lies inside the w x h image (Camera::inImage); otherwise out is left as it was.
+ALVA_CAM_FN bool rotate_prior(int lens, const double* K4, const double* D4, int w, int h, const double* R9, const double* bv,
+                              float* out) {
+    double c[3];
+    for (int i = 0; i < 3; i++) c[i] = (R9[i] * bv[0] + R9[3 + i] * bv[1]) + R9[6 + i] * bv[2];
+    if (!(c[2] > 0.0)) return false;
+    float o[2];
+    if (lens == 2) project_dist_fisheye(K4, D4, c, o);
+    else if (lens == 1) project_dist(K4, D4, c, o);
+    else project_pinhole(K4, c, o);
+    if (!(o[0] >= 0 && o[1] >= 0 && o[0] < w && o[1] < h)) return false;
+    out[0] = o[0];
+    out[1] = o[1];
+    return true;
+}
+
 }  // namespace alva_cam

@@ -25,6 +25,8 @@
 //                (not in the reference: alva_system_set_relocalisation)
 //   reacquire    fresh detections against the frozen map          alva_k_match_frame_to_map (reacquire.cu)
 //                (not in the reference: alva_system_set_localisation_only)
+//   klt_rotated  KLT's second pass with gyro-rotated priors          alva_k_rotate_priors (camera.cu) + alva_k_klt_fb
+//                (not in the reference: alva_system_set_gyro)
 // There is no CPU fallback: configure() fails without an sm_90 (H100) device.  Lens distortion: the JS shim always passes zeros
 // (system.js:84-141) and configure() rejects non-zero coefficients; setDistortion() (alva_system_set_distortion) sets them on a
 // configured System, and setFisheye() (alva_system_set_fisheye) selects OpenCV's equidistant fisheye model instead.  With a
@@ -46,6 +48,8 @@ int alva_undistort_points_launch(alva_ctx* ctx, const float* px, const int32_t* 
                                  const double* D4, float* unpx);
 int alva_undistort_points_fisheye_launch(alva_ctx* ctx, const float* px, const int32_t* counts, int nframes, int cap, const double* K4,
                                          const double* D4, float* unpx);
+int alva_rotate_priors_launch(alva_ctx* ctx, const double* bv, const uint8_t* flag, int n, int w, int h, const double* K4, const double* D4,
+                              int lens, const double* R9, float* prior, uint8_t* rotated);
 int alva_pose_chain_launch(alva_ctx* ctx, int n, int cap, const double* bvs, const double* X, const double* uv, const double* K4,
                            float fx, float fy, uint32_t seed, double* T12, double* info, uint8_t* o1, double* uv2, double* X2,
                            int32_t* n2, double* pose7, uint8_t* o2, double* summ, double huber, double chi2);
@@ -393,19 +397,39 @@ struct CudaBackend {
 
     // FeatureTracker::fbKltTracking(prev pyramid, cur pyramid, 9, levels, 30, 0.5, pts, priors, status)
     int klt(const float* pts, float* priors, int n, int levels, uint8_t* good) {
+        return klt_with(pts, priors, n, levels, good, nullptr, nullptr, nullptr, nullptr);
+    }
+    // the gyro mode's second pass (system_core.h kltTracking): alva_k_rotate_priors replaces the flagged priors on the device
+    // between the upload and alva_k_klt_fb -- one more launch, the same upload / download / synchronisation
+    int klt_rotated(const float* pts, float* priors, int n, int levels, uint8_t* good, const double* bv, const uint8_t* flag,
+                    const double* dR9, uint8_t* rotated) {
+        return klt_with(pts, priors, n, levels, good, bv, flag, dR9, rotated);
+    }
+    int klt_with(const float* pts, float* priors, int n, int levels, uint8_t* good, const double* bv, const uint8_t* flag,
+                 const double* dR9, uint8_t* rotated) {
         cudaStream_t st = ctx->stream;
         if (n > cap) { alva_set_error("System: %d keypoints exceed the frame capacity %d", n, cap); return ALVA_E_CAPACITY; }
         stg.reset();
         float *hp, *hq;
-        uint8_t* hg;
+        uint8_t *hg, *hf = nullptr, *hr = nullptr;
+        double* hb = nullptr;
         float* dp = stg.take<float>((size_t)2 * n, &hp);
+        double* db = bv ? stg.take<double>((size_t)3 * n, &hb) : nullptr;
+        uint8_t* df = bv ? stg.take<uint8_t>(n, &hf) : nullptr;
         float* dq = stg.take<float>((size_t)2 * n, &hq);
         const size_t q_off = (uint8_t*)dq - stg.d, up_end = stg.off;
         uint8_t* dg = stg.take<uint8_t>(n, &hg);
+        uint8_t* dr = bv ? stg.take<uint8_t>(n, &hr) : nullptr;
         float *hu = nullptr, *du = has_dist ? stg.take<float>((size_t)2 * n, &hu) : nullptr;   // the tracked points, undistorted
+        if (!stg.fits(stg.off)) { alva_set_error("System: staging buffer too small for %d points", n); return ALVA_E_CAPACITY; }
         memcpy(hp, pts, (size_t)n * 8);
         memcpy(hq, priors, (size_t)n * 8);
+        if (bv) { memcpy(hb, bv, (size_t)n * 24); memcpy(hf, flag, n); }
         SYS_CUDA(cudaMemcpyAsync(stg.d, stg.h, up_end, cudaMemcpyHostToDevice, st));
+        if (bv) {
+            const double K[4] = {fx, fy, cx, cy};
+            if (int e = alva_rotate_priors_launch(ctx, db, df, n, w, h, K, D4, fisheye ? 2 : (has_dist ? 1 : 0), dR9, dq, dr)) return e;
+        }
         const int prev = cur ^ 1;
         if (int e = alva_k_klt_fb(ctx, img[prev], der[prev], img[cur], der[cur], w, h, 1, nlev - 1, levels, 9, 30.0f, 0.5f, dp, dq, nullptr, n, dg))
             return e;
@@ -415,6 +439,7 @@ struct CudaBackend {
         SYS_CUDA(cudaStreamSynchronize(st));
         memcpy(priors, hq, (size_t)n * 8);
         memcpy(good, hg, n);
+        if (bv) memcpy(rotated, hr, n);
         if (has_dist) unpx_host.assign(hu, hu + 2 * (size_t)n);
         return 0;
     }
@@ -943,6 +968,24 @@ public:
         if (int e = core_.setLocalisationOnly(enabled != 0)) { alva_set_error("alva_system_set_localisation_only: %s", core_.map_error); return e; }
         return 0;
     }
+    // gyro-aided tracking (system_core.h setGyro): the state machine integrates the samples; the 2-D KLT priors are rotated on
+    // the device (CudaBackend::klt_rotated, alva_k_rotate_priors)
+    int setGyro(int enabled, const double* Rci, const double* bias) {
+        if (!configured_) { alva_set_error("System: not configured"); return ALVA_E_STATE; }
+        if (int e = core_.setGyro(enabled != 0, Rci, bias)) { alva_set_error("alva_system_set_gyro: %s", core_.map_error); return e; }
+        return 0;
+    }
+    int findCameraPoseGyro(const uint8_t* rgba, double t_ms, const double* samples, int n, float* pose16) {
+        if (!configured_) { alva_set_error("System: not configured"); return ALVA_E_STATE; }
+        if (int e = core_.addGyroSamples(samples, n)) { alva_set_error("alva_system_find_camera_pose_gyro: %s", core_.map_error); return e; }
+        return findCameraPose(rgba, t_ms, pose16);
+    }
+    int gyroStats(int32_t* out5, double* dR9) const {
+        out5[0] = core_.n_gyro_pred; out5[1] = core_.n_gyro_fallback; out5[2] = core_.n_gyro_carried; out5[3] = core_.n_gyro_rot;
+        out5[4] = core_.n_gyro_kept;
+        if (dR9) memcpy(dR9, core_.gyro_dRc, 9 * sizeof(double));
+        return 0;
+    }
     // {mode on, frames re-acquisition ran on, points it supplied, points of its last run}
     int localisationStats(int32_t* out4) const {
         out4[0] = core_.frozen ? 1 : 0; out4[1] = core_.n_reacq_runs; out4[2] = core_.n_reacq_points; out4[3] = core_.reacq_last_points;
@@ -1067,6 +1110,18 @@ extern "C" int alva_system_set_localisation_only(alva_system* s, int enabled) { 
 }
 extern "C" int alva_system_localisation_stats(alva_system* s, int32_t* out4) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
     return (s && out4) ? s->sys.localisationStats(out4) : ALVA_E_INVALID;
+}
+extern "C" int alva_system_set_gyro(alva_system* s, int enabled, const double* R_ci9, const double* bias3) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
+    if (!s || (enabled != 0 && enabled != 1)) { alva_set_error("alva_system_set_gyro: bad argument"); return ALVA_E_INVALID; }
+    return s->sys.setGyro(enabled, R_ci9, bias3);
+}
+extern "C" int alva_system_find_camera_pose_gyro(alva_system* s, const uint8_t* rgba, double t_ms, const double* samples, int n,
+                                                 float* pose16) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
+    if (!s || !rgba || !pose16) { alva_set_error("alva_system_find_camera_pose_gyro: bad argument"); return ALVA_E_INVALID; }
+    return s->sys.findCameraPoseGyro(rgba, t_ms, samples, n, pose16);
+}
+extern "C" int alva_system_gyro_stats(alva_system* s, int32_t* out5, double* dR9) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
+    return (s && out5) ? s->sys.gyroStats(out5, dR9) : ALVA_E_INVALID;
 }
 extern "C" int alva_system_save_map(alva_system* s, uint8_t* buf, size_t cap, size_t* bytes) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
     if (!s || !bytes) { alva_set_error("alva_system_save_map: bad argument"); return ALVA_E_INVALID; }

@@ -236,9 +236,11 @@ struct Camera {
             u = o[0]; v = o[1];
             return;
         }
-        const double iz = 1. / p[2];
-        const double x = (double)(float)(p[0] * iz), y = (double)(float)(p[1] * iz);
-        u = (float)(x * fx + cx); v = (float)(y * fy + cy);
+        double k[4];
+        float o[2];
+        K4(k);
+        alva_cam::project_pinhole(k, p, o);
+        u = o[0]; v = o[1];
     }
     bool inImage(float u, float v) const { return u >= 0 && v >= 0 && u < w && v < h; }
 };
@@ -481,6 +483,10 @@ template <class B> struct BackendHasReloc<B, std::void_t<decltype(std::declval<B
 template <class B, class = void> struct BackendHasReacquire : std::false_type {};
 template <class B> struct BackendHasReacquire<B, std::void_t<decltype(&B::reacquire)>> : std::true_type {};
 
+// a Backend may rotate the 2-D KLT priors by the gyroscope's rotation (klt_rotated); without it the gyro mode is refused
+template <class B, class = void> struct BackendHasRotatedKlt : std::false_type {};
+template <class B> struct BackendHasRotatedKlt<B, std::void_t<decltype(&B::klt_rotated)>> : std::true_type {};
+
 // ------------------------------------------------------------------------------------------------ flat problems handed to a Backend
 struct BaProblem {   // the layout of alva_k_ba_local
     int nkf = 0, nlm = 0, nobs = 0;
@@ -589,6 +595,10 @@ struct MapReader {
 //                 const uint8_t* qkept, int nq, float radius, int32_t* row, int32_t* dist)
 //                                                          alva_k_match_frame_to_map: per query the matched table row or -1
 //                                                          (localisation-only mode, reacquireFrame)
+//   int klt_rotated(const float* pts, float* priors, int n, int levels, uint8_t* good, const double* bv, const uint8_t* flag,
+//                   const double* dR9, uint8_t* rotated)   klt() after the prior of every flagged point is replaced by
+//                                                          alva_cam::rotate_prior of its bearing bv [n][3] under dR9 where that
+//                                                          is valid (rotated [n] = 1; the lens is the backend's) -- gyro mode
 //   optional: const float* unpx()                          see BackendHasUnpx
 template <class Backend>
 class SystemCore {
@@ -603,7 +613,85 @@ public:
         n_lens_drops = 0;
         setPreset(40, 0.95f, true);   // State(w, h, 40), mapKeyframeFilteringRatio_ 0.95, p3pEnabled_ (system.cpp:15-19)
         reloc_max = 0;
+        setGyro(false, nullptr, nullptr);
+        n_gyro_pred = n_gyro_fallback = n_gyro_carried = n_gyro_rot = n_gyro_kept = 0;
+        gyro_have_prev = false;
     }
+
+    // ------------------------------------------------------------------ gyro-aided tracking (not in the reference)
+    // The gyroscope's rotation between two frames predicts the camera's rotation, so a fast pan does not outrun the tracker.
+    //
+    // Samples {t_ms, gx, gy, gz (rad/s, IMU axes), ax, ay, az (ignored)} arrive with the frames (addGyroSamples) and are kept in
+    // time order.  After a frame at time t_k is integrated, every sample before the last one at or before t_k is discarded;
+    // samples later than t_k wait for the next frame.
+    //
+    // Integration over [A, B] = [t_{k-1}, t_k] (the previous and the current frame's time stamps, whatever their status):
+    //   omega(tau) at an end: with L the last sample at or before tau and H the first one after it, L + (H - L) (tau - t_L) /
+    //     (t_H - t_L) when both exist and t_H - t_L <= 50 ms; else L held when tau - t_L <= 50 ms; else H held when
+    //     t_H - tau <= 50 ms; else undefined.
+    //   breakpoints: A, the samples with A < t < B in order (each with its own omega: equal time stamps make zero-length
+    //     pieces), B.
+    //   covered: B >= A, a previous frame exists, omega is defined at both ends, and no two consecutive samples inside (A, B)
+    //     are more than 50 ms apart.
+    //   dR = I; per piece [a, b] in time order: dR <- dR Exp(((omega(a) + omega(b)) / 2 - bias) (b - a) / 1000), double
+    //     precision, Exp = Rodrigues (I + a K + b K^2, K = [phi]x; a = 1 - th^2 / 6, b = 1/2 - th^2 / 24 below th = 1e-6).
+    //   dR_c = R_ci dR R_ci^T: the rotation of the current camera in the previous one's axes (R_wc,k = R_wc,k-1 dR_c).
+    // A frame whose interval is not covered takes the camera-only path unchanged (counted in n_gyro_fallback).
+    //
+    // A covered frame:
+    //   - tracked (after the initialisation): the motion model's prediction keeps its translation, its rotation becomes
+    //     R_wc,k-1 dR_c; 3-D keypoints are projected with that pose as before (n_gyro_pred also counts covered frames before
+    //     the initialisation, whose pose is not predicted);
+    //   - KLT's second pass: every keypoint whose prior would be its previous position -- 2-D keypoints, 3-D keypoints whose
+    //     projection leaves the image, and all of them after a failed first pass -- starts from alva_cam::rotate_prior(dR_c,
+    //     bv) instead where that ray is in front of the camera and projects inside the image (n_gyro_rot), else from its
+    //     previous position (n_gyro_kept).  3-D keypoints that fail the first pass keep their projected prior;
+    //   - lost (relocalisation on, including the frame that loses the track): the pose keeps its translation and its rotation
+    //     advances by dR_c (n_gyro_carried); relocalisation itself uses no prior.
+    // setGyro needs a backend with klt_rotated (MAP_STATE otherwise).  R_ci (NULL: identity) takes IMU-axis vectors to camera
+    // axes; bias (NULL: zero) is a constant gyro bias in rad/s on the IMU axes.  A non-finite value, or an R_ci with an entry
+    // of R^T R - I above 1e-9 or a negative determinant, is refused (MAP_INVALID).  Disabling drops the samples.  configure
+    // ends the mode; reset, setPreset, setDistortion, setFisheye, setRelocalisation, setLocalisationOnly and loadMap keep it.
+    int setGyro(bool on, const double* Rci, const double* bias) {
+        if (!on) { gyro_on = gyro_ok = false; gyro_buf.clear(); gyroIdentity(gyro_dRc); return 0; }
+        double R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1}, b[3] = {0, 0, 0};
+        if (Rci) for (int i = 0; i < 9; i++) R[i] = Rci[i];
+        if (bias) for (int i = 0; i < 3; i++) b[i] = bias[i];
+        for (int i = 0; i < 9; i++) if (!std::isfinite(R[i])) { map_error = "non-finite R_ci"; return MAP_INVALID; }
+        for (int i = 0; i < 3; i++) if (!std::isfinite(b[i])) { map_error = "non-finite bias"; return MAP_INVALID; }
+        for (int i = 0; i < 3; i++)
+            for (int j = 0; j < 3; j++) {
+                const double d = R[i] * R[j] + R[3 + i] * R[3 + j] + R[6 + i] * R[6 + j] - (i == j ? 1.0 : 0.0);
+                if (!(fabs(d) <= 1e-9)) { map_error = "R_ci is not orthonormal"; return MAP_INVALID; }
+            }
+        const double det = R[0] * (R[4] * R[8] - R[5] * R[7]) - R[1] * (R[3] * R[8] - R[5] * R[6]) + R[2] * (R[3] * R[7] - R[4] * R[6]);
+        if (det < 0) { map_error = "R_ci is a reflection (negative determinant)"; return MAP_INVALID; }
+        if (!BackendHasRotatedKlt<Backend>::value) { map_error = "the backend cannot rotate KLT priors"; return MAP_STATE; }
+        memcpy(gyro_Rci, R, sizeof R);
+        memcpy(gyro_bias, b, sizeof b);
+        gyro_on = true;
+        return 0;
+    }
+
+    // samples [n][7] = {t_ms, gx, gy, gz, ax, ay, az} for the next frame.  Refused (MAP_INVALID, nothing kept) for n < 0, NULL
+    // with n > 0, a non-finite value, time stamps that decrease within the call or a sample older than the newest one held.
+    // Checked with the mode off too; kept only with it on.
+    int addGyroSamples(const double* s, int n) {
+        if (n < 0 || (!s && n > 0)) { map_error = "bad sample array"; return MAP_INVALID; }
+        double last = gyro_buf.empty() ? -INFINITY : gyro_buf.back().t;
+        for (int i = 0; i < n; i++) {
+            for (int c = 0; c < 7; c++) if (!std::isfinite(s[7 * (size_t)i + c])) { map_error = "non-finite sample"; return MAP_INVALID; }
+            if (s[7 * (size_t)i] < last) { map_error = "sample time stamps decrease"; return MAP_INVALID; }
+            last = s[7 * (size_t)i];
+        }
+        if (!gyro_on) return 0;
+        for (int i = 0; i < n; i++) {
+            const double* p = s + 7 * (size_t)i;
+            gyro_buf.push_back({p[0], {p[1], p[2], p[3]}});
+        }
+        return 0;
+    }
+    size_t gyroSamplesHeld() const { return gyro_buf.size(); }
 
     // relocalisation after a tracking loss (0 = off: the reference's reset on the fourth failed pose); kept by reset().  The
     // localisation-only mode needs it: turning it off then is refused (MAP_STATE).
@@ -780,6 +868,9 @@ public:
         cur.id++;
         cur.ts = timestamp;
         err = 0;
+        if (gyro_on) gyroFrame(timestamp);
+        gyro_prev_t = timestamp;
+        gyro_have_prev = true;
         bool kf = false;
         if (lost) {
             if constexpr (BackendHasReloc<Backend>::value) {
@@ -931,9 +1022,103 @@ public:
     // keypoints dropped because the fisheye model could not undistort them (tracked, detected or relocalisation queries), since
     // configure or the last lens change
     int n_lens_drops = 0;
+    // the gyro mode (setGyro): on, R_ci and bias; dR_c of the last frame integrated (identity when it was not covered); since
+    // configure: frames predicted from the gyro, frames that fell back to the motion model, lost frames whose rotation the
+    // gyro carried, 2-D priors rotated and 2-D priors kept at the previous position
+    bool gyro_on = false;
+    double gyro_Rci[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1}, gyro_bias[3] = {0, 0, 0};
+    double gyro_dRc[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+    int n_gyro_pred = 0, n_gyro_fallback = 0, n_gyro_carried = 0, n_gyro_rot = 0, n_gyro_kept = 0;
 
 private:
     Backend& B;
+    struct GyroSample { double t, w[3]; };
+    std::vector<GyroSample> gyro_buf;   // ascending t
+    bool gyro_ok = false;               // this frame's interval is covered: gyro_dRc holds its rotation
+    bool gyro_have_prev = false;
+    double gyro_prev_t = 0;             // the previous frame's time stamp
+
+    // ------------------------------------------------------------------ gyro integration (the rule: setGyro's comment)
+    static void gyroIdentity(double* R) { for (int i = 0; i < 9; i++) R[i] = (i % 4 == 0) ? 1.0 : 0.0; }
+    static void mul3(const double* A, const double* Bm, double* C) {
+        for (int i = 0; i < 3; i++)
+            for (int j = 0; j < 3; j++) C[3 * i + j] = (A[3 * i] * Bm[j] + A[3 * i + 1] * Bm[3 + j]) + A[3 * i + 2] * Bm[6 + j];
+    }
+    static void expSO3(const double* p, double* R) {
+        const double th2 = (p[0] * p[0] + p[1] * p[1]) + p[2] * p[2], th = sqrt(th2);
+        double a, b;
+        if (th < 1e-6) { a = 1.0 - th2 / 6.0; b = 0.5 - th2 / 24.0; }
+        else { a = sin(th) / th; b = (1.0 - cos(th)) / th2; }
+        // I + a [p]x + b [p]x^2, [p]x^2 = p p^T - th2 I
+        R[0] = 1.0 + b * (p[0] * p[0] - th2); R[1] = -a * p[2] + b * (p[0] * p[1]); R[2] = a * p[1] + b * (p[0] * p[2]);
+        R[3] = a * p[2] + b * (p[1] * p[0]); R[4] = 1.0 + b * (p[1] * p[1] - th2); R[5] = -a * p[0] + b * (p[1] * p[2]);
+        R[6] = -a * p[1] + b * (p[2] * p[0]); R[7] = a * p[0] + b * (p[2] * p[1]); R[8] = 1.0 + b * (p[2] * p[2] - th2);
+    }
+    size_t gyroUpper(double t) const {   // the first sample after t
+        return (size_t)(std::upper_bound(gyro_buf.begin(), gyro_buf.end(), t, [](double v, const GyroSample& s) { return v < s.t; }) - gyro_buf.begin());
+    }
+    bool gyroAt(double tau, double* w) const {
+        const size_t hi = gyroUpper(tau);
+        const GyroSample* L = hi > 0 ? &gyro_buf[hi - 1] : nullptr;
+        const GyroSample* H = hi < gyro_buf.size() ? &gyro_buf[hi] : nullptr;
+        if (L && H && H->t - L->t <= 50.0) {
+            const double f = (tau - L->t) / (H->t - L->t);
+            for (int c = 0; c < 3; c++) w[c] = L->w[c] + (H->w[c] - L->w[c]) * f;
+            return true;
+        }
+        if (L && tau - L->t <= 50.0) { for (int c = 0; c < 3; c++) w[c] = L->w[c]; return true; }
+        if (H && H->t - tau <= 50.0) { for (int c = 0; c < 3; c++) w[c] = H->w[c]; return true; }
+        return false;
+    }
+    bool gyroIntegrate(double A, double Bt, double* dR) const {
+        double wa[3], wb[3];
+        if (!(Bt >= A) || !gyroAt(A, wa) || !gyroAt(Bt, wb)) return false;
+        const size_t i0 = gyroUpper(A);
+        size_t i1 = i0;
+        while (i1 < gyro_buf.size() && gyro_buf[i1].t < Bt) i1++;
+        for (size_t i = i0 + 1; i < i1; i++) if (gyro_buf[i].t - gyro_buf[i - 1].t > 50.0) return false;
+        gyroIdentity(dR);
+        double ta = A;
+        const double* w0 = wa;
+        for (size_t i = i0; i <= i1; i++) {
+            const double tb = i < i1 ? gyro_buf[i].t : Bt;
+            const double* w1 = i < i1 ? gyro_buf[i].w : wb;
+            double phi[3], E[9], T[9];
+            for (int c = 0; c < 3; c++) phi[c] = ((w0[c] + w1[c]) / 2.0 - gyro_bias[c]) * ((tb - ta) / 1000.0);
+            expSO3(phi, E);
+            mul3(dR, E, T);
+            memcpy(dR, T, sizeof T);
+            ta = tb;
+            w0 = w1;
+        }
+        return true;
+    }
+    // the current frame: dR_c over [previous frame, this frame], the counters of the frames that fall back, and the samples
+    // no later frame needs
+    void gyroFrame(double t) {
+        double dR[9], T[9], Rt[9];
+        gyroIdentity(gyro_dRc);
+        gyro_ok = gyro_have_prev && gyroIntegrate(gyro_prev_t, t, dR);
+        if (gyro_ok) {
+            for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) Rt[3 * i + j] = gyro_Rci[3 * j + i];
+            mul3(gyro_Rci, dR, T);
+            mul3(T, Rt, gyro_dRc);
+        }
+        const bool tracking_path = lost || cur.id > 0;   // (a frame 0 starts the track: nothing to predict)
+        if (tracking_path && !gyro_ok) n_gyro_fallback++;
+        if (!lost && cur.id > 0 && gyro_ok) n_gyro_pred++;
+        const size_t hi = gyroUpper(t);
+        if (hi > 1) gyro_buf.erase(gyro_buf.begin(), gyro_buf.begin() + (hi - 1));
+    }
+    bool gyroUse() const { return gyro_on && gyro_ok; }
+    // prev with its rotation advanced by this frame's dR_c and the translation t
+    Se3 gyroRotated(const Se3& prev, const double* t) const {
+        Se3 D;
+        D.setR(gyro_dRc);
+        Se3 r = prev * D;
+        for (int i = 0; i < 3; i++) r.t[i] = t[i];
+        return r;
+    }
     MotionModel motion;
     bool p3p_req = false;
     bool reacq_pending = false;      // re-acquire on the next tracked frame (after freezing or a relocalisation)
@@ -1607,6 +1792,7 @@ private:
         Se3 Twc = cur.Twc;
         const Se3 tracked = cur.Twc;
         motion.apply(Twc, timestamp);
+        if (gyroUse() && ready_for_init) Twc = gyroRotated(tracked, Twc.t);   // the gyro's rotation, the motion model's translation
         cur.setTwc(Twc);
         kltTracking();
         if (err) return false;
@@ -1617,7 +1803,11 @@ private:
         }
         const bool ok = computePose();
         if (err) return false;
-        if (!ok && reloc_max > 0 && BackendHasReloc<Backend>::value) { enterLost(tracked); return false; }
+        if (!ok && reloc_max > 0 && BackendHasReloc<Backend>::value) {
+            if (gyroUse()) { enterLost(gyroRotated(tracked, tracked.t)); n_gyro_carried++; }
+            else enterLost(tracked);
+            return false;
+        }
         if (!ok) {
             pose_failed++;
             if (pose_failed > 3) { reset_requested = true; return false; }
@@ -1707,8 +1897,9 @@ private:
         reloc_last_matches = R.n_match;
         reloc_last_inliers = ok ? n2 - nout2 : 0;
         if (!ok) {
-            if (frozen) { if (lost_frames < INT32_MAX) lost_frames++; return 4; }   // a frozen map is never reset
+            if (frozen) { if (lost_frames < INT32_MAX) lost_frames++; gyroCarry(); return 4; }   // a frozen map is never reset
             if (++lost_frames > reloc_max) { reset(); return 2; }
+            gyroCarry();
             return 4;
         }
         // the PnP inliers become the frame's keypoints, observing their map points
@@ -1732,6 +1923,13 @@ private:
         if (frozen) { reacq_pending = true; return 1; }   // no keyframe; the next tracked frame re-acquires
         kf = checkNewKeyframeRequired();
         return 1;
+    }
+
+    // a lost frame with the gyro: the reported pose turns with the camera, its translation held
+    void gyroCarry() {
+        if (!gyroUse()) return;
+        cur.setTwc(gyroRotated(cur.Twc, cur.Twc.t));
+        n_gyro_carried++;
     }
 
     // ------------------------------------------------------------------ re-acquisition (localisation only)
@@ -1803,6 +2001,15 @@ private:
     void kltTracking() {   // kltTrackingFromMotionPrior (kltUsePrior_ = true)
         std::vector<int> ids3, ids;
         std::vector<float> kps3, pri3, kps, pri;
+        // gyro mode: per second-pass point its bearing and whether its prior is the previous position (then rotated)
+        const bool rot = gyroUse();
+        std::vector<double> bvs;
+        std::vector<uint8_t> rflag;
+        auto second = [&](const Keypoint& k, bool prev_prior) {
+            if (!rot) return;
+            bvs.insert(bvs.end(), k.bv, k.bv + 3);
+            rflag.push_back(prev_prior ? 1 : 0);
+        };
         ids3.reserve(cur.n3d); kps3.reserve(2 * (size_t)cur.n3d); pri3.reserve(2 * (size_t)cur.n3d);
         ids.reserve(cur.n); kps.reserve(2 * (size_t)cur.n); pri.reserve(2 * (size_t)cur.n);
         double Rcw[9];
@@ -1822,6 +2029,7 @@ private:
                 }
             }
             ids.push_back(k.id); kps.push_back(k.px); kps.push_back(k.py); pri.push_back(k.px); pri.push_back(k.py);
+            second(k, true);
         }
         if (!ids3.empty()) {
             const size_t n3 = ids3.size();
@@ -1833,14 +2041,26 @@ private:
             for (size_t i = 0; i < n3; i++) {
                 if (good[i] && lensDrop(pri3[2 * i], pri3[2 * i + 1], un ? un + 2 * i : nullptr)) { removeObsFromCurr(ids3[i]); continue; }
                 if (good[i]) { cur.update(ids3[i], pri3[2 * i], pri3[2 * i + 1], un ? un + 2 * i : nullptr); ngood++; }
-                else { ids.push_back(ids3[i]); kps.push_back(kps3[2 * i]); kps.push_back(kps3[2 * i + 1]); pri.push_back(pri3[2 * i]); pri.push_back(pri3[2 * i + 1]); }
+                else {
+                    ids.push_back(ids3[i]); kps.push_back(kps3[2 * i]); kps.push_back(kps3[2 * i + 1]); pri.push_back(pri3[2 * i]); pri.push_back(pri3[2 * i + 1]);
+                    if (rot) second(*cur.find(ids3[i]), false);   // (not updated: still the previous frame's keypoint)
+                }
             }
-            if (ngood < 0.33 * n3) { p3p_req = true; pri = kps; }
+            if (ngood < 0.33 * n3) { p3p_req = true; pri = kps; rflag.assign(rflag.size(), 1); }   // the rotation is trusted still
         }
         if (!ids.empty()) {
             const size_t n = ids.size();
             std::vector<uint8_t> good(n);
-            if ((err = B.klt(kps.data(), pri.data(), (int)n, 3, good.data())) < 0) return;   // State::kltPyramidLevels_
+            if (rot) {
+                std::vector<uint8_t> rotated(n);
+                if constexpr (BackendHasRotatedKlt<Backend>::value)   // (the mode is refused without it)
+                    if ((err = B.klt_rotated(kps.data(), pri.data(), (int)n, 3, good.data(), bvs.data(), rflag.data(), gyro_dRc, rotated.data())) < 0)
+                        return;
+                for (size_t i = 0; i < n; i++)
+                    if (rflag[i]) { if (rotated[i]) n_gyro_rot++; else n_gyro_kept++; }
+            } else if ((err = B.klt(kps.data(), pri.data(), (int)n, 3, good.data())) < 0) {   // State::kltPyramidLevels_
+                return;
+            }
             err = 0;
             const float* un = backendUnpx();
             for (size_t i = 0; i < n; i++) {

@@ -74,6 +74,7 @@ _OPTIONAL = {
                                   _vp, _vp, _i32, _vp, _vp, _vp, C.c_float, _vp, _vp],
     "alva_k_undistort_points_fisheye": [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp],
     "alva_k_project_points_fisheye": [_vp, _vp, _i32, _vp, _vp, _vp],
+    "alva_k_rotate_priors": [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _i32, _vp, _vp, _vp],
     "alva_k_p3p_lmeds": [_vp, _i32, _i32, _vp, _vp, _vp, _i32, C.c_float, C.c_float, C.c_float, C.c_uint32, _vp, _vp, _vp],
     "alva_k_p3p_ransac": [_vp, _i32, _i32, _vp, _vp, _vp, _i32, C.c_float, C.c_float, C.c_float, C.c_uint32, _vp, _vp, _vp],
     "alva_k_hamming_knn2_grouped": [_vp, _vp, _i32, _vp, _i32, _vp, _i32, _vp],
@@ -275,6 +276,13 @@ class Context:
     def project_points_fisheye(self, Xc, n, K, k4, uv):
         """cv::fisheye::projectPoints of the float points (x/z, y/z, 1) -- see alva_k_project_points_fisheye."""
         self._chk(self.L.alva_k_project_points_fisheye(self.h, _ptr(Xc), n, _f64x4(K), _f64x4(k4), _ptr(uv)))
+
+    def rotate_priors(self, bv, flag, n, w, h, K, D4, lens, R9, prior, rotated):
+        """System's gyro-rotated KLT priors -- see alva_k_rotate_priors; K / D4 (None: zeros) / R9 on the host, lens 0 pinhole,
+        1 radial-tangential, 2 fisheye."""
+        R = (C.c_double * 9)(*[float(v) for v in R9])
+        self._chk(self.L.alva_k_rotate_priors(self.h, _ptr(bv), _ptr(flag), n, w, h, _f64x4(K), None if D4 is None else _f64x4(D4), lens, R,
+                                              _ptr(prior), _ptr(rotated)))
 
     def p3p_lmeds(self, nprob, cap, bvs, wpts, counts, Twc_out, outlier, info=None, max_iter=100, err_px=3.0, fx=1.0, fy=1.0,
                   seed=12345):

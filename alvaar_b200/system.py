@@ -27,6 +27,9 @@ def _bind():
     L.alva_system_load_map.argtypes = [_vp, C.c_char_p, C.c_size_t]
     L.alva_system_set_localisation_only.argtypes = [_vp, _i32]
     L.alva_system_localisation_stats.argtypes = [_vp, _vp]
+    L.alva_system_set_gyro.argtypes = [_vp, _i32, _vp, _vp]
+    L.alva_system_find_camera_pose_gyro.argtypes = [_vp, _vp, _f64, _vp, _i32, _vp]
+    L.alva_system_gyro_stats.argtypes = [_vp, _vp, _vp]
     L.alva_system_num_matched.argtypes = [_vp]
     L.alva_system_configure.argtypes = [_vp, _i32, _i32] + [_f64] * 8
     L.alva_system_find_camera_pose.argtypes = [_vp, _vp, _vp]
@@ -244,3 +247,41 @@ class System:
         o = np.zeros(4, np.int32)
         self.L.alva_system_localisation_stats(self.h, o.ctypes.data_as(_vp))
         return dict(zip(("on", "runs", "points", "last"), o.tolist()))
+
+    def set_gyro(self, enabled=True, R_ci=None, bias=None):
+        """Gyro-aided tracking: the gyroscope's rotation between frames predicts the camera's, so fast pans keep tracking.
+        Samples then come with the frames through find_camera_pose_gyro().  R_ci (3x3, default identity) takes IMU-axis
+        vectors to camera axes -- diag(1, -1, -1) for the W3C devicemotion rotationRate axes and a rear camera; bias (3, rad/s
+        on the IMU axes, default zero) is subtracted from every sample.  enabled=False turns it off and drops the samples
+        held.  Survives reset(), set_preset(), set_clahe(), set_distortion(), set_fisheye(), set_relocalisation(),
+        set_localisation_only() and load_map(); a new System starts with it off.  AlvaError (nothing changed) for a
+        non-finite value or an R_ci that is not a rotation."""
+        R = None if R_ci is None else np.ascontiguousarray(R_ci, np.float64).reshape(9)
+        b = None if bias is None else np.ascontiguousarray(bias, np.float64).reshape(3)
+        rc = self.L.alva_system_set_gyro(self.h, 1 if enabled else 0, None if R is None else R.ctypes.data_as(_vp),
+                                         None if b is None else b.ctypes.data_as(_vp))
+        if rc != 0:
+            raise AlvaError(f"alva_system_set_gyro -> {rc}: {self.L.alva_last_error().decode()}")
+
+    def find_camera_pose_gyro(self, rgba, t_ms, samples):
+        """find_camera_pose with gyro samples -> (status, pose[16]).  samples: [n, 7] rows {t_ms, gx, gy, gz (rad/s), ax, ay,
+        az} (the reference's IMU layout; the accelerometer columns are ignored), in time order, none older than the samples
+        already given; samples later than t_ms are kept for the next frame.  With set_gyro off they are checked and ignored.
+        AlvaError (no frame processed) for a refused sample array."""
+        self._check(rgba)
+        s = np.ascontiguousarray(samples, np.float64).reshape(-1, 7)
+        pose = np.zeros(16, np.float32)
+        st = self.L.alva_system_find_camera_pose_gyro(self.h, rgba.ctypes.data_as(_vp), float(t_ms), s.ctypes.data_as(_vp) if len(s) else None,
+                                                      len(s), pose.ctypes.data_as(_vp))
+        if st < 0:
+            raise AlvaError(f"alva_system_find_camera_pose_gyro -> {st}: {self.L.alva_last_error().decode()}")
+        return st, pose
+
+    def gyro_stats(self):
+        """-> ({"predicted": frames whose rotation came from the gyro, "fallback": frames whose interval the samples did not
+        cover, "carried": lost frames whose rotation the gyro advanced, "rotated" / "kept": KLT priors rotated / kept at the
+        previous position}, dR [3, 3]: the last frame's camera rotation from the gyro, identity when not covered)"""
+        o = np.zeros(5, np.int32)
+        dR = np.zeros(9)
+        self.L.alva_system_gyro_stats(self.h, o.ctypes.data_as(_vp), dR.ctypes.data_as(_vp))
+        return dict(zip(("predicted", "fallback", "carried", "rotated", "kept"), o.tolist())), dR.reshape(3, 3)

@@ -108,6 +108,16 @@ int alva_k_project_points(alva_ctx*, const double* Xc, int n, const double* K4, 
 int alva_k_undistort_points_fisheye(alva_ctx*, const float* px, const int32_t* counts, int nframes, int cap, const double* K4,
                                     const double* D4, float* unpx);
 int alva_k_project_points_fisheye(alva_ctx*, const double* Xc, int n, const double* K4, const double* D4, float* uv);
+/* The rotation-compensated KLT priors of System's gyro mode (alva_system_set_gyro; not in the reference).  For every point i with
+ * flag[i] != 0: c = R^T bv[i] (bv [n][3] double, the keypoint's bearing in the previous camera; R9 row-major, the camera's
+ * rotation from the previous frame to the current one, HOST array), projected through the lens -- 0 the pinhole, 1 the
+ * radial-tangential model (alva_k_project_points), 2 the fisheye model (alva_k_project_points_fisheye) -- and written to
+ * prior [n][2] float (8-byte aligned) with rotated[i] = 1 only when c.z > 0 and the projection lies inside the w x h image
+ * (0 <= u < w, 0 <= v < h).  Every other point keeps its prior, with rotated[i] = 0.  K4 / D4 / R9 are host arrays (D4 NULL:
+ * zeros); bv, flag, prior, rotated are device arrays; n = 0 is a no-op.  Bit-exact with the host build of the same arithmetic
+ * (camera_model.h).  ALVA_E_INVALID for a bad pointer, size or lens, a zero focal length or a non-finite coefficient. */
+int alva_k_rotate_priors(alva_ctx*, const double* bv, const uint8_t* flag, int n, int w, int h, const double* K4, const double* D4,
+                         int lens, const double* R9, float* prior, uint8_t* rotated);
 
 /* cv::FAST(gray, thr, nms=true, TYPE_9_16) on each frame (opencv features2d/src/fast.cpp:496).
  * keys[f*cap + i]: packed corner keys; counts[f] = true number found (may exceed cap: then only cap
@@ -560,6 +570,38 @@ int  alva_system_set_localisation_only(alva_system*, int enabled);
 /* out4 = {mode on, frames re-acquisition ran on, map points it returned to the frame, those of its last run}, since the
  * handle was created */
 int  alva_system_localisation_stats(alva_system*, int32_t* out4);
+/* Gyro-aided tracking: the gyroscope's rotation between two frames predicts the camera's, so a fast pan (which a 9x9 KLT
+ * without a rotation prior loses within a few frames) keeps tracking.  enabled = 1 turns it on; samples then come with the
+ * frames through alva_system_find_camera_pose_gyro.
+ *   R_ci9: row-major rotation taking IMU-axis vectors to camera axes (omega_c = R_ci omega_i); NULL = identity.  For the W3C
+ *          `devicemotion` rotationRate axes (x right, y up, z out of the screen) and a rear camera (x right, y down, z forward)
+ *          it is diag(1, -1, -1).
+ *   bias3: a constant gyro bias in rad/s on the IMU axes, subtracted from every sample; NULL = zero.
+ * Between the previous and the current frame's time stamps omega is taken piecewise linear between samples and integrated
+ * piece by piece in double precision (the exact rule is in alvaar_b200/csrc/system_core.h, SystemCore::setGyro).  An interval
+ * is covered when omega is known at both ends (interpolated, or held from a sample at most 50 ms away) and no two samples
+ * inside it are more than 50 ms apart; a frame whose interval is not covered is tracked exactly as without the mode.  On a
+ * covered frame: the motion model's predicted rotation is replaced by the gyro's (its translation kept); every KLT prior that
+ * would start at the keypoint's previous position starts at the projection of its bearing turned by that rotation (on the
+ * device, alva_k_rotate_priors), where that lies in front of the camera and inside the image; and a lost frame (relocalisation
+ * on) reports its last pose turned by the rotation, its translation held -- pose16 and a map saved while lost carry it.
+ * enabled = 0 turns it off and drops the samples held.  configure clears it; reset, set_preset, set_clahe, set_distortion,
+ * set_fisheye, set_relocalisation, set_localisation_only and load_map keep it.  ALVA_E_STATE before configure;
+ * ALVA_E_INVALID for a null handle, enabled other than 0 / 1, a non-finite value, or an R_ci that is not a rotation (an
+ * entry of R^T R - I above 1e-9 in magnitude, or a negative determinant).  A refusal changes nothing. */
+int  alva_system_set_gyro(alva_system*, int enabled, const double* R_ci9, const double* bias3);
+/* alva_system_find_camera_pose_ts with gyro samples.  samples [n][7] in the reference's per-sample layout {t_ms, gx, gy, gz
+ * (rad/s), ax, ay, az}: the tail of its JS shim's IMU buffer can be passed unchanged; the accelerometer fields are ignored.
+ * Samples may run ahead of t_ms: they are kept for the next frame.  With the mode off the samples are checked and ignored and
+ * the call equals alva_system_find_camera_pose_ts bit for bit.  Refused with ALVA_E_INVALID -- no frame processed, nothing
+ * changed -- for n < 0, samples NULL with n > 0, a non-finite value, time stamps that decrease within the call, or a sample
+ * older than the newest one the handle holds (equal time stamps are allowed: Date.now() has a 1 ms resolution). */
+int  alva_system_find_camera_pose_gyro(alva_system*, const uint8_t* rgba, double t_ms, const double* samples, int n, float* pose16);
+/* out5 = {frames whose rotation was predicted from the gyro, frames that fell back to the motion model (interval not
+ * covered), lost frames whose rotation the gyro carried, KLT priors rotated, KLT priors kept at the previous position
+ * (rotated ray behind the camera or outside the image)}, since configure; dR9 (may be NULL) = the last frame's rotation
+ * dR_c = R_ci dR R_ci^T, row-major (identity when its interval was not covered). */
+int  alva_system_gyro_stats(alva_system*, int32_t* out5, double* dR9);
 /* The map as a self-contained byte string, to resume a session in a new handle or to start another stream in this one's map and
  * coordinate frame.
  *

@@ -56,6 +56,9 @@ public:
     // not in the reference's class: track against the map without changing it (alva_system_set_localisation_only); needs
     // setRelocalisation > 0 and a map (loaded or initialised); loadMap keeps it on.  0 or an ALVA_E_* code
     int setLocalisationOnly(bool enabled) { return alva_system_set_localisation_only(h_, enabled ? 1 : 0); }
+    // not in the reference's class: gyro-aided tracking (alva_system_set_gyro); R_ci9 (row-major IMU -> camera axes, NULL:
+    // identity; diag(1, -1, -1) for devicemotion and a rear camera) and bias3 (rad/s, NULL: zero).  0 or an ALVA_E_* code
+    int setGyro(int enabled, const double* R_ci9 = nullptr, const double* bias3 = nullptr) { return alva_system_set_gyro(h_, enabled, R_ci9, bias3); }
 
     // ---- the reference's wasm32 signatures
     int findCameraPose(int imageRGBADataPtr, int posePtr) { return findCameraPose(ptr<const uint8_t>(imageRGBADataPtr), ptr<float>(posePtr)); }
@@ -72,6 +75,11 @@ public:
     }
     int findCameraPoseWithIMU(const uint8_t* imageRGBA, const double* imuData, float* pose16) {
         return alva_system_find_camera_pose_imu(h_, imageRGBA, imuData, pose16);
+    }
+    // not in the reference's class: findCameraPose with n gyro samples [n][7] = {t_ms, gx, gy, gz, ax, ay, az} (the JS shim's
+    // IMU buffer layout) for setGyro's mode; with the mode off it equals findCameraPose(imageRGBA, timestampMs, pose16)
+    int findCameraPoseWithGyro(const uint8_t* imageRGBA, double timestampMs, const double* samples, int n, float* pose16) {
+        return alva_system_find_camera_pose_gyro(h_, imageRGBA, timestampMs, samples, n, pose16);
     }
     int findPlane(float* location16, int numIterations) { return alva_system_find_plane(h_, location16, numIterations); }
     int getFramePoints(int32_t* pointsXY) { return alva_system_get_frame_points(h_, pointsXY, 2048); }
