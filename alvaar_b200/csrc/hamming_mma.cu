@@ -17,10 +17,12 @@
 //                       hands the ring stage back, and runs the top-2 selection on the accumulators in its own registers
 //                       while the other warpgroups' MMAs keep the tensor cores busy.  In the accumulator fragment a thread
 //                       holds 32 columns of two rows; it reduces every 8 dot products of a row to their maximum and compares
-//                       it with the dot product of its current second best; only the groups that hit run the top-2
-//                       insertion, on packed keys hamming << 22 | index (one multiply-add builds a key, three min / max insert
-//                       it: OpenCV's strict '<' with ties to the lowest train index is the unsigned order of those keys).  The
-//                       four threads that share a row merge their pairs by shuffles at the end.
+//                       the largest of the four with a bound on the row's second best, which the four threads of the row
+//                       share by shuffles once per tile; only the groups above it run the top-2 insertion, on packed keys
+//                       hamming << 22 | index (one multiply-add builds a key, three min / max insert it: OpenCV's strict
+//                       '<' with ties to the lowest train index is the unsigned order of those keys).  The selection, not
+//                       the MMAs, bounds the kernel (DESIGN §4.4), so its cost per tile is what these filters cut.  The four
+//                       threads that share a row merge their pairs by shuffles at the end.
 //   warp 16     producer: bulk async copies (cp.async.bulk, the TMA engine's 1-D mode) of pre-tiled 32 KB operand blobs into
 //                       a 4-stage shared-memory ring, completion on mbarriers.
 // The operands are expanded from the packed 256-bit descriptors by knn2_expand_kernel straight into the shared-memory
@@ -220,6 +222,68 @@ __device__ __forceinline__ void merge2(uint32_t& k0, uint32_t& k1, uint32_t o0, 
     k1 = min(min(k1, o1), hi);
 }
 
+// Top-2 selection over the accumulators of one 64 x 128 tile, n0 = train row of the thread's first column.  Per thread and
+// row: the two smallest keys seen, key = hamming << 22 | index = (256 - dot) << 21 | index -- the lexicographic (distance,
+// index) order of OpenCV's insertion as ONE unsigned compare, so the insertion itself is three min / max and needs no order
+// of arrival.  thr = a dot product the row's final second best is known to reach: a candidate can only matter if its dot
+// product is strictly above it (its index is larger than everything that set the bound).  The row's 32 dot products of the
+// thread are compared as a whole first, then in groups of 8, and only groups above thr run the insertion.  TAIL: the last
+// train tile, whose columns past nt must not be inserted.
+// fragment: d[4c + 2h + e] = D[r0 + 8h][8c + 2 quad + e], c < 16
+template <class A, bool TAIL>
+__device__ __forceinline__ void top2_rows(const typename A::T (&d)[64], int n0, int nt, uint32_t (&k0)[2], uint32_t (&k1)[2],
+                                          typename A::T (&thr)[2]) {
+    using T = typename A::T;
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+        // The four threads of a row share their bounds: a thread's second best is a candidate of the row, so the row's final
+        // second best is at least as good, and every column of this tile has a larger index than the earlier tiles' columns.
+        thr[h] = max(thr[h], __shfl_xor_sync(0xffffffffu, thr[h], 1));
+        thr[h] = max(thr[h], __shfl_xor_sync(0xffffffffu, thr[h], 2));
+        T gmax[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) {                         // 8 columns of row r0 + 8h: c = 4k .. 4k + 3, e = 0, 1
+            gmax[k] = d[16 * k + 2 * h];
+#pragma unroll
+            for (int c = 0; c < 4; c++)
+#pragma unroll
+                for (int e = 0; e < 2; e++) gmax[k] = max(gmax[k], d[16 * k + 4 * c + 2 * h + e]);
+        }
+        if (max(max(gmax[0], gmax[1]), max(gmax[2], gmax[3])) <= thr[h]) continue;
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            if (gmax[k] > thr[h]) {
+#pragma unroll
+                for (int c = 0; c < 4; c++) {
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        const int col = n0 + 8 * (4 * k + c) + e;
+                        const uint32_t key = !TAIL || col < nt ? A::key(d[16 * k + 4 * c + 2 * h + e], col) : NONE;
+                        const uint32_t hi = max(k0[h], key);
+                        k0[h] = min(k0[h], key);
+                        k1[h] = min(k1[h], hi);
+                    }
+                }
+                thr[h] = max(thr[h], A::dot_of_key(k1[h]));
+            }
+        }
+    }
+}
+
+// top2_rows over the tile whose first column is train row col0
+template <class A>
+__device__ __forceinline__ void top2_tile(typename A::T (&d)[64], int col0, int quad, int nt, uint32_t (&k0)[2],
+                                          uint32_t (&k1)[2], typename A::T (&thr)[2]) {
+    const int n0 = col0 + 2 * quad;
+    if (col0 + TN > nt) {                                     // only the last train tile: columns past nt hold zero rows
+#pragma unroll
+        for (int i = 0; i < 64; i++) if (n0 + 8 * (i >> 2) + (i & 1) >= nt) d[i] = A::neg();   // never opens a group
+        top2_rows<A, true>(d, n0, nt, k0, k1, thr);
+    } else {
+        top2_rows<A, false>(d, n0, nt, k0, k1, thr);
+    }
+}
+
 template <int KIND>
 __global__ void __launch_bounds__(NTHREADS, 1)
 knn2_mma_kernel(const uint8_t* __restrict__ Aexp, const uint8_t* __restrict__ Bexp, const int32_t* __restrict__ rowmap,
@@ -272,11 +336,7 @@ knn2_mma_kernel(const uint8_t* __restrict__ Aexp, const uint8_t* __restrict__ Be
     const int quad = lane & 3;
     const int trow = (g & 1) * WM + (warp & 3) * 16 + (lane >> 2);   // row inside the A tile of accumulator row r0; r1 = r0 + 8
     const uint32_t a0 = smem_u32(sA) + (uint32_t)t * BLOB + (uint32_t)(g & 1) * L.moff;
-    // Per thread and row: the two smallest keys seen, key = hamming << 22 | index = (256 - dot) << 21 | index -- the
-    // lexicographic (distance, index) order of OpenCV's insertion as ONE unsigned compare, so the insertion itself is three
-    // min / max and needs no order of arrival.  thr = the dot product of the current second best: a candidate can only
-    // matter if its dot product is strictly above it (its index is larger than everything this thread has seen).
-    uint32_t k0[2] = {NONE, NONE}, k1[2] = {NONE, NONE};
+    uint32_t k0[2] = {NONE, NONE}, k1[2] = {NONE, NONE};   // per row r0, r0 + 8: the two smallest keys (top2_tile)
     T thr[2] = {A::neg(), A::neg()};
     T d[64];
 #pragma unroll
@@ -301,36 +361,7 @@ knn2_mma_kernel(const uint8_t* __restrict__ Aexp, const uint8_t* __restrict__ Be
 #pragma unroll
             for (int i = 0; i < 64; i++) dbg[(trow + 8 * ((i >> 1) & 1)) * TN + 8 * (i >> 2) + 2 * quad + (i & 1)] = A::to_int(d[i]);
         }
-        const int n0 = (tile0 + it) * TN + 2 * quad;
-        if (n0 - 2 * quad + TN > nt) {                        // only the last train tile: columns past nt hold zero rows
-#pragma unroll
-            for (int i = 0; i < 64; i++) if (n0 + 8 * (i >> 2) + (i & 1) >= nt) d[i] = A::neg();   // never opens a group
-        }
-#pragma unroll
-        for (int h = 0; h < 2; h++) {
-#pragma unroll
-            for (int k = 0; k < 4; k++) {                     // 8 columns of row r0 + 8h: c = 4k .. 4k + 3, e = 0, 1
-                T gmax = d[16 * k + 2 * h];
-#pragma unroll
-                for (int c = 0; c < 4; c++)
-#pragma unroll
-                    for (int e = 0; e < 2; e++) gmax = max(gmax, d[16 * k + 4 * c + 2 * h + e]);
-                if (gmax > thr[h]) {
-#pragma unroll
-                    for (int c = 0; c < 4; c++) {
-#pragma unroll
-                        for (int e = 0; e < 2; e++) {
-                            const int col = n0 + 8 * (4 * k + c) + e;
-                            const uint32_t key = col < nt ? A::key(d[16 * k + 4 * c + 2 * h + e], col) : NONE;
-                            const uint32_t hi = max(k0[h], key);
-                            k0[h] = min(k0[h], key);
-                            k1[h] = min(k1[h], hi);
-                        }
-                    }
-                    thr[h] = A::dot_of_key(k1[h]);
-                }
-            }
-        }
+        top2_tile<A>(d, (tile0 + it) * TN, quad, nt, k0, k1, thr);
     }
     // merge the four threads of a row (lanes 4 j .. 4 j + 3 hold disjoint columns of the same two rows)
 #pragma unroll
