@@ -48,6 +48,8 @@ struct DetectParams {
     int out_cap;
     float sp_mask[49];       // cornerSubPix Gaussian window (host expf)
     int32_t* dbg;            // optional [8] counters (ALVA_DETECT_DEBUG): why the select kernel re-scanned a cell
+    uint8_t* sel;            // [nframes][sel_bytes]: the select kernel's prim / sec / cell states when they do not fit in shared memory
+    size_t sel_bytes;
 };
 
 __device__ __forceinline__ int refl(int p, int n) {
@@ -85,9 +87,10 @@ __global__ void __launch_bounds__(512) detect_prepare_kernel(const DetectParams 
     const int lane = tid & 31, wid = tid >> 5, nw = blockDim.x >> 5;
     for (int i = wid; i < n; i += nw) {
         const float px = cur[2 * i], py = cur[2 * i + 1];
-        // occupiedCells[px.y / cellSize][px.x / cellSize] (float division, truncation to size_t)
+        // occupiedCells[px.y / cellSize][px.x / cellSize] (float division, truncation to size_t: a quotient in (-1, 0), i.e. a
+        // coordinate in (-cell, 0), truncates to row / column 0; below that the conversion is undefined and nothing is marked)
         const float fr = py / (float)P.cs, fc = px / (float)P.cs;
-        if (lane == 0 && fr >= 0.f && fc >= 0.f) {
+        if (lane == 0 && fr > -1.f && fc > -1.f) {
             const long long r = (long long)fr, c = (long long)fc;
             if (r <= P.nch && c <= P.ncw) occ[r * (P.ncw + 1) + c] = 1;
         }
@@ -209,6 +212,9 @@ __global__ void __launch_bounds__(256) detect_mineig_kernel(const DetectParams P
 // Everything a cell needs in the common case is in shared memory: its two pre-computed maxima and the detections of the
 // four neighbours processed before it.  Only when a neighbour's disc covers a pre-computed maximum is the cell re-scanned
 // (static bit mask AND the neighbouring / own discs); nothing is written to HBM until the final list.
+// A grid too large for shared memory (kGlobalSel) keeps prim / sec / cell states in the workspace (P.sel) and reads the
+// pre-computed maxima where the cell kernel left them; the arithmetic and the order are the same.
+template <bool kGlobalSel>
 __global__ void __launch_bounds__(512) detect_select_kernel(const DetectParams P) {
     extern __shared__ int32_t sel[];      // prim[ncells], sec[ncells]  (x | y << 16, -1 = none), then float4 cand[ncells], occ bytes
     __shared__ int s_nocc;
@@ -216,10 +222,12 @@ __global__ void __launch_bounds__(512) detect_select_kernel(const DetectParams P
     const int f = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, nw = blockDim.x >> 5;
     const int cs = P.cs, ncells = P.nch * P.ncw;
     if (tid <= MAX_RADIUS) shw[tid] = P.hw[tid];
-    int32_t* prim = sel;
-    int32_t* sec = sel + ncells;
-    float4* cand = reinterpret_cast<float4*>(sel + 2 * ncells + ((2 * ncells) & 3 ? 4 - ((2 * ncells) & 3) : 0));
-    uint8_t* socc = reinterpret_cast<uint8_t*>(cand + ncells);
+    int32_t* const base = kGlobalSel ? reinterpret_cast<int32_t*>(P.sel + (size_t)f * P.sel_bytes) : sel;
+    int32_t* prim = base;
+    int32_t* sec = base + ncells;
+    float4* scand = reinterpret_cast<float4*>(sel + 2 * ncells + ((2 * ncells) & 3 ? 4 - ((2 * ncells) & 3) : 0));
+    const float4* cand = kGlobalSel ? P.cand + (size_t)f * ncells : scand;
+    uint8_t* socc = kGlobalSel ? reinterpret_cast<uint8_t*>(base + 2 * ncells) : reinterpret_cast<uint8_t*>(scand + ncells);
     const uint8_t* occ = P.occ + (size_t)f * (P.nch + 1) * (P.ncw + 1);
     const double q = P.quality[f];
     if (tid == 0) s_nocc = 0;
@@ -233,7 +241,7 @@ __global__ void __launch_bounds__(512) detect_select_kernel(const DetectParams P
         socc[i] = o ? 1 : (searched ? 0 : 2);
         myocc += o ? 1 : 0;
         prim[i] = -1; sec[i] = -1;
-        if (searched) cand[i] = P.cand[(size_t)f * ncells + i];
+        if (!kGlobalSel && searched) scand[i] = P.cand[(size_t)f * ncells + i];
     }
     if (myocc) atomicAdd(&s_nocc, myocc);
     __syncthreads();
@@ -501,7 +509,12 @@ extern "C" int alva_k_detect_grid(alva_ctx* ctx, const uint8_t* gray, int w, int
     const size_t hmap_b = (size_t)nframes * ncells * cell * cell * sizeof(float);
     const size_t mask_b = (size_t)nframes * h * P.mw * sizeof(uint32_t);
     const size_t cand_b = (size_t)nframes * ncells * sizeof(float4);
-    const size_t need = occ_b + hmap_b + mask_b + cand_b + 1024;
+    // the select kernel keeps its per-cell state in shared memory up to 200 KB (8 191 cells), in the workspace past that
+    const size_t sm2 = (size_t)2 * ncells * sizeof(int32_t) + 16 + (size_t)ncells * (sizeof(float4) + 1);
+    const bool sel_global = sm2 > 200 * 1024;
+    P.sel_bytes = sel_global ? ((size_t)ncells * (2 * sizeof(int32_t) + 1) + 15) & ~(size_t)15 : 0;
+    const size_t sel_b = (size_t)nframes * P.sel_bytes;
+    const size_t need = occ_b + hmap_b + mask_b + cand_b + 1024 + (sel_global ? sel_b + 256 : 0);
     if (need > ctx->det_ws_bytes) {
         ctx->ws_epoch++;
         if (ctx->det_ws) { ALVA_CUDA(cudaStreamSynchronize(ctx->stream)); ALVA_CUDA(cudaFree(ctx->det_ws)); ctx->det_ws = nullptr; ctx->det_ws_bytes = 0; }
@@ -511,6 +524,7 @@ extern "C" int alva_k_detect_grid(alva_ctx* ctx, const uint8_t* gray, int w, int
     uint8_t* ws = (uint8_t*)ctx->det_ws;
     P.occ = ws; P.hmap = (float*)(ws + occ_b); P.mask = (uint32_t*)(ws + occ_b + hmap_b);
     P.cand = (float4*)(ws + ((occ_b + hmap_b + mask_b + 255) & ~(size_t)255));
+    if (sel_global) P.sel = ws + ((((occ_b + hmap_b + mask_b + 255) & ~(size_t)255) + cand_b + 255) & ~(size_t)255);
     P.quality = quality; P.out = out; P.out_int = out_int; P.counts = counts; P.out_cap = out_cap;
     static int32_t* dbg_dev = nullptr;
     static const bool dbg_on = getenv("ALVA_DETECT_DEBUG") != nullptr;
@@ -525,10 +539,11 @@ extern "C" int alva_k_detect_grid(alva_ctx* ctx, const uint8_t* gray, int w, int
     ALVA_CUDA(cudaFuncSetAttribute(detect_mineig_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm1));
     detect_mineig_kernel<<<dim3(ncells, nframes), 256, sm1, ctx->stream>>>(P);
     ALVA_LAUNCH_CHECK(ctx);
-    const size_t sm2 = (size_t)2 * ncells * sizeof(int32_t) + 16 + (size_t)ncells * (sizeof(float4) + 1);
-    if (sm2 > 200 * 1024) { alva_set_error("alva_k_detect_grid: too many cells (%d)", ncells); return ALVA_E_INVALID; }
-    ALVA_CUDA(cudaFuncSetAttribute(detect_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm2));
-    detect_select_kernel<<<nframes, 512, sm2, ctx->stream>>>(P);
+    if (sel_global) detect_select_kernel<true><<<nframes, 512, 0, ctx->stream>>>(P);
+    else {
+        ALVA_CUDA(cudaFuncSetAttribute(detect_select_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm2));
+        detect_select_kernel<false><<<nframes, 512, sm2, ctx->stream>>>(P);
+    }
     ALVA_LAUNCH_CHECK(ctx);
     corner_subpix_kernel<<<dim3((out_cap + 63) / 64, nframes), 64, 0, ctx->stream>>>(P, out, counts, out_cap, 30, 0.01 * 0.01);
     ALVA_LAUNCH_CHECK(ctx);

@@ -193,7 +193,9 @@ int alva_k_hamming_knn2_grouped(alva_ctx*, const uint8_t* q, int nq, const int32
  *   be NULL); roi (HOST) = {x, y, width, height} (CameraCalibration's border rect, 20 px); quality [nframes] double IN/OUT =
  *   maxQuality_ (0.001 at start, system.cpp:29); out [nframes][out_cap][2] float sub-pixel corners; out_int (optional)
  *   [nframes][out_cap][2] int32 the integer maxima before refinement; counts [nframes] (true count; only out_cap are stored).
- * 8 <= cell <= 64 (the reference uses 40).  Bit-identical to the reference run with cv::setNumThreads(1). */
+ * 8 <= cell <= 64 (the reference uses 40), any grid the frame size allows.  A current keypoint in (-cell, 0) marks row /
+ * column 0 occupied, as the reference's truncating cell index does.  Bit-identical to the reference run with
+ * cv::setNumThreads(1). */
 int alva_k_detect_grid(alva_ctx*, const uint8_t* gray, int w, int h, int nframes, int cell, const float* cur,
                        const int32_t* ncur, int cur_cap, const int32_t* roi, double* quality, float* out, int32_t* out_int,
                        int32_t* counts, int out_cap);
