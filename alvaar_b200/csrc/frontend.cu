@@ -884,15 +884,18 @@ __global__ void __launch_bounds__(256) pyrdown_kernel(const uint8_t* __restrict_
 }
 
 // ---- restore cv::FAST's row-major order: bucket by row, then sort each row's few keys by x ---------
-__global__ void __launch_bounds__(1024) order_keys_kernel(const uint32_t* __restrict__ in, uint32_t* __restrict__ out,
-                                                          const int32_t* __restrict__ counts, int cap, int h) {
+// The first min(counts[f], cap) keys of `in` are ordered into `work` (same stride cap).  When `out` is another buffer, the
+// first out_cap of the ordered keys are then copied there (stride out_cap): a truncation in row-major order, the same on every
+// run.  out_counts (optional, may alias counts) receives min(count, cap, out_cap).
+__global__ void __launch_bounds__(1024) order_keys_kernel(const uint32_t* __restrict__ in, uint32_t* work, const int32_t* counts,
+                                                          int cap, int h, uint32_t* out, int32_t* out_counts, int out_cap) {
     extern __shared__ int osm[];   // rowstart[h+1], rowfill[h]
     int* rowstart = osm;
     int* rowfill = osm + h + 1;
     const int f = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
     const int n = min(counts[f], cap);
     const uint32_t* kin = in + (size_t)f * cap;
-    uint32_t* kout = out + (size_t)f * cap;
+    uint32_t* kout = work + (size_t)f * cap;
     for (int i = tid; i <= h; i += nt) rowstart[i] = 0;
     for (int i = tid; i < h; i += nt) rowfill[i] = 0;
     __syncthreads();
@@ -932,13 +935,21 @@ __global__ void __launch_bounds__(1024) order_keys_kernel(const uint32_t* __rest
             kout[j + 1] = k;
         }
     }
+    const int nout = min(n, out_cap);
+    if (out != work) {
+        __syncthreads();
+        uint32_t* dst = out + (size_t)f * out_cap;
+        for (int i = tid; i < nout; i += nt) dst[i] = kout[i];
+    }
+    if (out_counts && tid == 0) out_counts[f] = nout;   // every thread read counts[f] before the first barrier
 }
 
 // ---- KeyPointsFilter::retainBest on packed keys (one CTA per frame) --------------------------------
+// Every kept key is written (out has the input's stride cap, and at most min(count, cap) keys are kept), in atomic order;
+// out_counts[f] = the kept count.  order_keys_kernel then orders them and truncates.
 __global__ void __launch_bounds__(1024) retain_best_kernel(const uint32_t* __restrict__ in, const int32_t* __restrict__ counts,
                                                            int cap, int w, int h, int n_keep, int edge,
-                                                           uint32_t* __restrict__ out, int32_t* __restrict__ out_counts,
-                                                           int out_cap) {
+                                                           uint32_t* __restrict__ out, int32_t* __restrict__ out_counts) {
     __shared__ int hist[256];
     __shared__ int thr_s, cnt_s;
     const int f = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
@@ -973,13 +984,10 @@ __global__ void __launch_bounds__(1024) retain_best_kernel(const uint32_t* __res
     }
     __syncthreads();
     const int thr = thr_s;
-    uint32_t* kout = out + (size_t)f * out_cap;
+    uint32_t* kout = out + (size_t)f * cap;
     for (int i = tid; i < n; i += nt) {
         const uint32_t k = kin[i];
-        if (inside(k) && (int)(k & 255) >= thr) {
-            const int pos = atomicAdd(&cnt_s, 1);
-            if (pos < out_cap) kout[pos] = k;
-        }
+        if (inside(k) && (int)(k & 255) >= thr) kout[atomicAdd(&cnt_s, 1)] = k;
     }
     __syncthreads();
     if (tid == 0) out_counts[f] = cnt_s;
@@ -1136,10 +1144,12 @@ static int launch_pyrdown(alva_ctx* ctx, const uint8_t* src, uint8_t* dst, int w
     return 0;
 }
 
-static int launch_order(alva_ctx* ctx, const uint32_t* in, uint32_t* out, const int32_t* counts, int cap, int h,
-                        int nframes) {
+// in -> work (both stride cap) in row-major order; then, if out != work, its first out_cap keys -> out (stride out_cap).
+// out_counts (optional) = the counts clamped to cap and out_cap.
+static int launch_order(alva_ctx* ctx, const uint32_t* in, uint32_t* work, const int32_t* counts, int cap, int h, int nframes,
+                        uint32_t* out, int32_t* out_counts, int out_cap) {
     const size_t smem = (size_t)(2 * h + 1) * sizeof(int);
-    order_keys_kernel<<<nframes, 1024, smem, ctx->stream>>>(in, out, counts, cap, h);
+    order_keys_kernel<<<nframes, 1024, smem, ctx->stream>>>(in, work, counts, cap, h, out, out_counts, out_cap);
     ALVA_LAUNCH_CHECK(ctx);
     return 0;
 }
@@ -1212,7 +1222,7 @@ static int fast_common(alva_ctx* ctx, bool rgba_mode, const uint8_t* src, int w,
         }
     }
     if (keys && sorted)
-        if (int e = launch_order(ctx, raw, keys, counts, cap, h, nframes)) return e;
+        if (int e = launch_order(ctx, raw, keys, counts, cap, h, nframes, keys, nullptr, cap)) return e;
     return 0;
 }
 
@@ -1234,11 +1244,16 @@ extern "C" int alva_k_retain_best(alva_ctx* ctx, const uint32_t* keys, const int
         alva_set_error("alva_k_retain_best: bad argument");
         return ALVA_E_INVALID;
     }
-    uint32_t* tmp = (uint32_t*)alva_scratch(ctx, (size_t)nframes * out_cap * sizeof(uint32_t));
+    // select every kept key (up to cap of them) into tmp, order them all, then keep the first out_cap: the truncation never
+    // depends on the order in which the selection's atomics land.  With out_cap == cap the ordering writes out_keys directly.
+    const bool direct = out_cap == cap;
+    const size_t words = (size_t)nframes * cap;
+    uint32_t* tmp = (uint32_t*)alva_scratch(ctx, (direct ? 1 : 2) * words * sizeof(uint32_t));
     if (!tmp) return ALVA_E_CUDA;
-    retain_best_kernel<<<nframes, 1024, 0, ctx->stream>>>(keys, counts, cap, w, h, n, edge, tmp, out_counts, out_cap);
+    uint32_t* work = direct ? out_keys : tmp + words;
+    retain_best_kernel<<<nframes, 1024, 0, ctx->stream>>>(keys, counts, cap, w, h, n, edge, tmp, out_counts);
     ALVA_LAUNCH_CHECK(ctx);
-    return launch_order(ctx, tmp, out_keys, out_counts, out_cap, h, nframes);
+    return launch_order(ctx, tmp, work, out_counts, cap, h, nframes, out_keys, out_counts, out_cap);
 }
 
 // Host-buffer front end: pinned/pageable host RGBA in, packed keys + counts out.  The copies are part of the call

@@ -476,7 +476,8 @@ extern "C" int alva_k_orb_detect(alva_ctx* ctx, const uint8_t* gray, int w, int 
         alva_set_error("alva_k_orb_detect: bad argument (need w, h >= 64)");
         return ALVA_E_INVALID;
     }
-    const int kcap = (int)std::min<size_t>(std::max<size_t>(8192, (size_t)w * h / 24), 1u << 20);
+    // every FAST corner fits: the strict 3x3 NMS leaves at most one per 2x2 block
+    const int kcap = ((w + 1) / 2) * ((h + 1) / 2);
     auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
     const size_t b_keys = al((size_t)nframes * kcap * 4), b_pts = al((size_t)nframes * kcap * 8), b_resp = al((size_t)nframes * kcap * 4);
     const size_t b_cnt = al((size_t)nframes * 4), b_img = al((size_t)nframes * w * h);

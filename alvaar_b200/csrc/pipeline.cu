@@ -7,6 +7,7 @@
 // feature front end; `System` (system.cu) drives it one frame at a time, bench.py drives it in batches.
 #include "alva_common.cuh"
 #include "../../include/alva_b200.h"
+#include <algorithm>
 #include <map>
 #include <tuple>
 #include <vector>
@@ -17,19 +18,23 @@ extern "C" int alva_k_hamming_knn2_batch(alva_ctx*, const uint8_t* q, const int3
 
 namespace {
 
+// grid-stride over the slots: a pre-selection list's capacity (the NMS bound of the frame) is far larger than its live count
 __global__ void keys_to_points_kernel(const uint32_t* __restrict__ keys, const int32_t* __restrict__ counts, int cap,
                                       float* __restrict__ pts, int live_only) {
-    const int f = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= cap) return;
+    const int f = blockIdx.y;
     const int n = min(counts[f], cap);
-    if (live_only && i >= n) return;   // large pre-selection lists: dead slots are never read
-    float2 p = make_float2(0.f, 0.f);
-    if (i < n) {
-        const uint32_t k = keys[(size_t)f * cap + i];
-        p = make_float2((float)ALVA_KEY_X(k), (float)ALVA_KEY_Y(k));
+    const int end = live_only ? n : cap;   // large pre-selection lists: dead slots are never read
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < end; i += gridDim.x * blockDim.x) {
+        float2 p = make_float2(0.f, 0.f);
+        if (i < n) {
+            const uint32_t k = keys[(size_t)f * cap + i];
+            p = make_float2((float)ALVA_KEY_X(k), (float)ALVA_KEY_Y(k));
+        }
+        reinterpret_cast<float2*>(pts)[(size_t)f * cap + i] = p;
     }
-    reinterpret_cast<float2*>(pts)[(size_t)f * cap + i] = p;
 }
+
+static unsigned points_blocks(int cap) { return (unsigned)std::min((cap + 127) / 128, 32); }
 
 __global__ void clamp_counts_kernel(int32_t* counts, int n, int cap) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -42,7 +47,7 @@ struct alva_pipeline {
     alva_ctx* ctx = nullptr;
     alva_pipeline_config cfg{};
     int w1, h1, w2, h2, w3, h3;
-    int kcap = 32768;   // raw FAST corners per frame
+    int kcap = 0;       // raw FAST corners per frame: the NMS bound, so that none is ever dropped
     int fcap = 0;       // selected features per frame (slots)
     int nprob = 0;      // BA problems per step
     // device buffers
@@ -181,7 +186,8 @@ extern "C" alva_pipeline* alva_pipeline_create(alva_ctx* ctx, const alva_pipelin
     p->w1 = (w + 1) / 2; p->h1 = (h + 1) / 2; p->w2 = (p->w1 + 1) / 2; p->h2 = (p->h1 + 1) / 2;
     p->w3 = (p->w2 + 1) / 2; p->h3 = (p->h2 + 1) / 2;
     p->fcap = ((cfg->nfeatures + cfg->nfeatures / 2 + 63) / 64) * 64;   // retainBest keeps ties: 1.5x head-room
-    p->kcap = (w * h) / 16 > 32768 ? (w * h) / 16 : 32768;
+    // FAST's 3x3 NMS is strict, so no two corners are neighbours: at most one per 2x2 block.  Every corner of a frame fits.
+    p->kcap = ((w + 1) / 2) * ((h + 1) / 2);
     p->nprob = cfg->kf_interval > 0 ? (B + cfg->kf_interval - 1) / cfg->kf_interval : 0;
     PALLOC(l0, (size_t)B * w * h); PALLOC(l1, (size_t)B * p->w1 * p->h1); PALLOC(l2, (size_t)B * p->w2 * p->h2);
     PALLOC(l3, (size_t)B * p->w3 * p->h3); PALLOC(blur, (size_t)B * w * h);
@@ -335,9 +341,7 @@ static int pipeline_frames(alva_pipeline* p, const uint8_t* rgba_dev, int f0, in
         int32_t* counts2 = p->counts2 + F;
         float *pts2 = p->pts2 + F * p->kcap * 2, *resp2 = p->resp2 + F * p->kcap;
         if (int e = alva_k_retain_best(sc, keys, counts, p->kcap, nf, w, h, 2 * c.nfeatures, 31, keys2, counts2, p->kcap)) return e;
-        clamp_counts_kernel<<<(nf + 127) / 128, 128, 0, ss>>>(counts2, nf, p->kcap);
-        ALVA_LAUNCH_CHECK(sc);
-        keys_to_points_kernel<<<dim3((p->kcap + 127) / 128, nf), 128, 0, ss>>>(keys2, counts2, p->kcap, pts2, 1);
+        keys_to_points_kernel<<<dim3(points_blocks(p->kcap), nf), 128, 0, ss>>>(keys2, counts2, p->kcap, pts2, 1);
         ALVA_LAUNCH_CHECK(sc);
         if (int e = alva_harris_launch(sc, l0, w, h, nf, pts2, counts2, p->kcap, resp2, 0)) return e;
         if (int e = alva_retain_best_f32_launch(sc, pts2, resp2, counts2, p->kcap, nf, c.nfeatures, p->pts + F * p->fcap * 2, keys2, sel,
@@ -346,10 +350,9 @@ static int pipeline_frames(alva_pipeline* p, const uint8_t* rgba_dev, int f0, in
         clamp_counts_kernel<<<(nf + 127) / 128, 128, 0, ss>>>(selcounts, nf, p->fcap);
         ALVA_LAUNCH_CHECK(sc);
     } else {
+        // retainBest keeps ties, so more than fcap can survive: the call keeps the first fcap of them in row-major order
         if (int e = alva_k_retain_best(sc, keys, counts, p->kcap, nf, w, h, c.nfeatures, 31, sel, selcounts, p->fcap)) return e;
-        clamp_counts_kernel<<<(nf + 127) / 128, 128, 0, ss>>>(selcounts, nf, p->fcap);
-        ALVA_LAUNCH_CHECK(sc);
-        keys_to_points_kernel<<<dim3((p->fcap + 127) / 128, nf), 128, 0, ss>>>(sel, selcounts, p->fcap, p->pts + F * p->fcap * 2, 0);
+        keys_to_points_kernel<<<dim3(points_blocks(p->fcap), nf), 128, 0, ss>>>(sel, selcounts, p->fcap, p->pts + F * p->fcap * 2, 0);
         ALVA_LAUNCH_CHECK(sc);
     }
     ALVA_CUDA(cudaEventRecord(p->sel_join, ss));

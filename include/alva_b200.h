@@ -119,9 +119,11 @@ int alva_k_project_points_fisheye(alva_ctx*, const double* Xc, int n, const doub
 int alva_k_rotate_priors(alva_ctx*, const double* bv, const uint8_t* flag, int n, int w, int h, const double* K4, const double* D4,
                          int lens, const double* R9, float* prior, uint8_t* rotated);
 
-/* cv::FAST(gray, thr, nms=true, TYPE_9_16) on each frame (opencv features2d/src/fast.cpp:496).
- * keys[f*cap + i]: packed corner keys; counts[f] = true number found (may exceed cap: then only cap
- * are stored and the call returns ALVA_E_CAPACITY after completing).  sorted != 0: row-major order. */
+/* cv::FAST(gray, thr, nms=true, TYPE_9_16) on each frame (opencv features2d/src/fast.cpp:496); thr is clamped to 0..255 as
+ * cv::FAST does.  Asynchronous on the context's stream.  keys[f*cap + i]: packed corner keys; counts[f] = the true number found.
+ * It may exceed cap: then cap of the corners are stored, and which ones is unspecified (the caller compares counts[f] with cap;
+ * a cap of ceil(w/2) * ceil(h/2), the bound of the strict 3x3 NMS, never overflows).  sorted != 0: the stored keys in
+ * row-major order. */
 int alva_k_fast9(alva_ctx*, const uint8_t* gray, int w, int h, int nframes, int thr,
                  uint32_t* keys, int32_t* counts, int cap, int sorted);
 
@@ -134,7 +136,9 @@ int alva_k_frontend(alva_ctx*, const uint8_t* rgba, int w, int h, int nframes,
 
 /* KeyPointsFilter::retainBest(n) on FAST keys (features2d/src/keypoint.cpp:69-90): keeps every corner
  * whose score >= the n-th best score (ties can make it more than n), border-filtered like ORB
- * (edge = 31: orb.cpp:1130) when edge > 0; result sorted row-major.  out_counts[f] <= out_cap. */
+ * (edge = 31: orb.cpp:1130) when edge > 0, of the first min(counts[f], cap) keys; result sorted row-major.  When more than
+ * out_cap are kept, the first out_cap in row-major order are stored (the same on every call): out_counts[f] =
+ * min(kept, out_cap).  n < 0 keeps every key inside the border; n = 0 none. */
 int alva_k_retain_best(alva_ctx*, const uint32_t* keys, const int32_t* counts, int cap, int nframes,
                        int w, int h, int n, int edge, uint32_t* out_keys, int32_t* out_counts, int out_cap);
 
@@ -159,7 +163,7 @@ int alva_k_harris(alva_ctx*, const uint8_t* gray, int w, int h, int nframes, con
  * :785-958): FAST(fast_thr, nms) -> border 31 -> retainBest(2*nfeatures) on the FAST score -> Harris -> retainBest(nfeatures)
  * on the Harris response (ties kept, so counts can exceed nfeatures) -> IC angle -> blur -> steered rBRIEF.
  * kp_out [nframes][out_cap][4] float = {x, y, Harris response, angle in degrees}; desc [nframes][out_cap][32];
- * counts[f] = keypoints found (only the first out_cap are stored).  Order: row-major (y, x) -- the reference's order is
+ * counts[f] = keypoints found (the first out_cap in row-major order are stored).  Order: row-major (y, x) -- the reference's order is
  * whatever std::nth_element leaves, so compare as sets.  flags: ALVA_ORB_FMA selects the blur arithmetic. */
 int alva_k_orb_detect(alva_ctx*, const uint8_t* gray, int w, int h, int nframes, int nfeatures, int fast_thr, int flags,
                       float* kp_out, uint8_t* desc, int32_t* counts, int out_cap);
@@ -445,7 +449,10 @@ typedef struct alva_pipeline alva_pipeline;
 typedef struct alva_pipeline_config {
     int w, h, batch;        /* frame geometry and frames per step */
     int fast_thr;           /* FAST threshold (ORB default 20) */
-    int nfeatures;          /* retainBest target per frame */
+    int nfeatures;          /* retainBest target per frame.  Ties at the n-th best can keep more; a frame has
+                               fcap = 1.5 * nfeatures rounded up to 64 feature slots (alva_pipeline_info), and a selection
+                               larger than that keeps its first fcap in row-major order.  Every FAST corner of a frame is a
+                               candidate (the key capacity is the NMS bound, ceil(w/2) * ceil(h/2)). */
     int orb_flags;          /* ALVA_ORB_* */
     int map_size;           /* descriptors in the local map (0 = no matching) */
     int kf_interval;        /* one local BA per kf_interval frames (0 = no BA) */
