@@ -1,4 +1,5 @@
-// camera_model.h -- the radial-tangential lens model (k1, k2, p1, p2) of the reference's CameraCalibration, in one place for
+// camera_model.h -- the radial-tangential lens model (k1, k2, p1, p2) of the reference's CameraCalibration, OpenCV's full
+// 14-coefficient form of it (k3..k6, the thin prism s1..s4 and the tilt tau_x, tau_y) and its fisheye model, in one place for
 // the host state machine (system_core.h), the kernels (camera.cu, match.cu) and the CPU System backend of the test suite.
 //
 // The reference stores its coefficients as an Eigen::Vector4d, so its cv::Mat copy is never empty and it always runs OpenCV
@@ -9,13 +10,16 @@
 //                    result stays in pixels
 //   project_dist     CameraCalibration::projectCamToImageDist -> cv::projectPoints of the FLOAT point (x/z, y/z, 1) with zero
 //                    rvec / tvec = cvProjectPoints2Internal (opencv calib3d/src/calibration.cpp:526-810, distortion :780-803)
-// Both are restated in OpenCV's expression order, with its 14-coefficient array (the 10 unused entries are zeros that still
-// take part in the arithmetic: 0 * inf is NaN, -0 + 0 is +0) and its identity tilt and rotation matrices multiplied out as
+// Both are restated in OpenCV's expression order, with its 14-coefficient array (entries a four-coefficient lens does not use
+// are zeros that still take part in the arithmetic: 0 * inf is NaN, -0 + 0 is +0) and its tilt and rotation matrices multiplied out as
 // Matx::operator* accumulates (s = 0; s += a(i, k) * b(k), core/matx.hpp:860-870).  Bit-exact only without FMA contraction:
 // device users compile with -fmad=false, host users with -ffp-contract=off.
 //
-// Both take K4 = {fx, fy, cx, cy} and D4 = {k1, k2, p1, p2}.
+// The 14-coefficient forms (undistort_point_full, project_dist_full) take the whole vector and the two tilt matrices, which the
+// host builds once per lens (make_lens_full); undistort_point / project_dist take K4 = {fx, fy, cx, cy} and D4 = {k1, k2, p1, p2}
+// and call them with ten zeros and the identity.
 #pragma once
+#include <math.h>
 
 #if defined(__CUDACC__)
 #define ALVA_CAM_FN __host__ __device__ inline
@@ -25,19 +29,30 @@
 
 namespace alva_cam {
 
-// out = cv::undistortPoints of the float pixel (u, v), rounded to float
-ALVA_CAM_FN void undistort_point(const double* K4, const double* D4, float u_in, float v_in, float* out) {
-    const double k[14] = {D4[0], D4[1], D4[2], D4[3], 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+constexpr double kHalfPi = 1.57079632679489661923;   // CV_PI / 2.
+
+// OpenCV's full pinhole distortion vector: k[14] = {k1, k2, p1, p2, k3, k4, k5, k6, s1, s2, s3, s4, tau_x, tau_y} (the 4-, 5-, 8-
+// and 12-entry vectors of cv::calibrateCamera are its prefixes, zero-padded), with the two tilt matrices of
+// detail::computeTiltProjectionMatrix (tilt_matrices below, host only) row-major.  Passed by value into the kernels.
+struct LensFull {
+    double k[14];
+    double tilt[9];    // matTilt, what projectPoints applies
+    double itilt[9];   // invMatTilt, what undistortPoints applies
+};
+
+// out = cv::undistortPoints of the float pixel (u, v), rounded to float; k: the 14 coefficients, invMatTilt: row-major 3x3
+ALVA_CAM_FN void undistort_point_full(const double* K4, const double* k, const double* invMatTilt, float u_in, float v_in, float* out) {
+    const double* M = invMatTilt;
     const double fx = K4[0], fy = K4[1], cx = K4[2], cy = K4[3];
     const double ifx = 1. / fx, ify = 1. / fy;
     double x = u_in, y = v_in;
     const double u = x, v = y;
     x = (x - cx) * ifx;
     y = (y - cy) * ify;
-    // invMatTilt (identity) * (x, y, 1)                                                                            :482-486
-    const double t0 = ((0. + 1. * x) + 0. * y) + 0. * 1.;
-    const double t1 = ((0. + 0. * x) + 1. * y) + 0. * 1.;
-    const double t2 = ((0. + 0. * x) + 0. * y) + 1. * 1.;
+    // invMatTilt * (x, y, 1)                                                                                       :482-486
+    const double t0 = ((0. + M[0] * x) + M[1] * y) + M[2] * 1.;
+    const double t1 = ((0. + M[3] * x) + M[4] * y) + M[5] * 1.;
+    const double t2 = ((0. + M[6] * x) + M[7] * y) + M[8] * 1.;
     const double invProj = t2 ? 1. / t2 : 1;
     const double x0 = x = invProj * t0;
     const double y0 = y = invProj * t1;
@@ -62,9 +77,10 @@ ALVA_CAM_FN void undistort_point(const double* K4, const double* D4, float u_in,
     out[1] = (float)(yy * ww);
 }
 
-// out = cv::projectPoints of the camera-frame point p through cv::Point3f(p.x / p.z, p.y / p.z, 1), rounded to float
-ALVA_CAM_FN void project_dist(const double* K4, const double* D4, const double* p, float* out) {
-    const double k[14] = {D4[0], D4[1], D4[2], D4[3], 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+// out = cv::projectPoints of the camera-frame point p through cv::Point3f(p.x / p.z, p.y / p.z, 1), rounded to float; k: the 14
+// coefficients, matTilt: row-major 3x3
+ALVA_CAM_FN void project_dist_full(const double* K4, const double* k, const double* matTilt, const double* p, float* out) {
+    const double* M = matTilt;
     const double fx = K4[0], fy = K4[1], cx = K4[2], cy = K4[3];
     const double inverseZ = 1. / p[2];
     const double X = (float)(p[0] * inverseZ), Y = (float)(p[1] * inverseZ), Z = 1.0f;   // camera_calibration.cpp:36-46
@@ -80,14 +96,67 @@ ALVA_CAM_FN void project_dist(const double* K4, const double* D4, const double* 
     const double icdist2 = 1. / (1 + k[5] * r2 + k[6] * r4 + k[7] * r6);
     const double xd0 = x * cdist * icdist2 + k[2] * a1 + k[3] * a2 + k[8] * r2 + k[9] * r4;
     const double yd0 = y * cdist * icdist2 + k[2] * a3 + k[3] * a1 + k[10] * r2 + k[11] * r4;
-    // matTilt (identity) * (xd0, yd0, 1)                                                                           :803-806
-    const double t0 = ((0. + 1. * xd0) + 0. * yd0) + 0. * 1.;
-    const double t1 = ((0. + 0. * xd0) + 1. * yd0) + 0. * 1.;
-    const double t2 = ((0. + 0. * xd0) + 0. * yd0) + 1. * 1.;
+    // matTilt * (xd0, yd0, 1)                                                                                      :803-806
+    const double t0 = ((0. + M[0] * xd0) + M[1] * yd0) + M[2] * 1.;
+    const double t1 = ((0. + M[3] * xd0) + M[4] * yd0) + M[5] * 1.;
+    const double t2 = ((0. + M[6] * xd0) + M[7] * yd0) + M[8] * 1.;
     const double invProj = t2 ? 1. / t2 : 1;
     const double xd = invProj * t0, yd = invProj * t1;
     out[0] = (float)(xd * fx + cx);                                                                                 // :808-809, :1010
     out[1] = (float)(yd * fy + cy);
+}
+
+// the four-coefficient model: the 14-entry array with ten literal zeros and the literal identity tilt
+ALVA_CAM_FN void undistort_point(const double* K4, const double* D4, float u_in, float v_in, float* out) {
+    const double k[14] = {D4[0], D4[1], D4[2], D4[3], 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+    const double eye[9] = {1., 0., 0., 0., 1., 0., 0., 0., 1.};
+    undistort_point_full(K4, k, eye, u_in, v_in, out);
+}
+ALVA_CAM_FN void project_dist(const double* K4, const double* D4, const double* p, float* out) {
+    const double k[14] = {D4[0], D4[1], D4[2], D4[3], 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+    const double eye[9] = {1., 0., 0., 0., 1., 0., 0., 0., 1.};
+    project_dist_full(K4, k, eye, p, out);
+}
+
+// detail::computeTiltProjectionMatrix<double>(tauX, tauY) (imgproc/src/distortion_model.hpp:75-123) for matTilt and invMatTilt,
+// in Matx's accumulation order; both the identity unless tau_x or tau_y is non-zero, as cvUndistortPointsInternal and
+// cvProjectPoints2Internal build them.  Host only (no __device__): glibc's cos / sin are OpenCV's, the device's round differently.
+inline void matx33_mul(const double* a, const double* b, double* c) {
+    for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++) {
+            double s = 0;
+            for (int l = 0; l < 3; l++) s += a[3 * i + l] * b[3 * l + j];
+            c[3 * i + j] = s;
+        }
+}
+inline void tilt_matrices(double tauX, double tauY, double* matTilt, double* invMatTilt) {
+    for (int i = 0; i < 9; i++) matTilt[i] = invMatTilt[i] = (i % 4 == 0) ? 1. : 0.;
+    if (!(tauX != 0 || tauY != 0)) return;
+    const double cTauX = cos(tauX), sTauX = sin(tauX), cTauY = cos(tauY), sTauY = sin(tauY);
+    const double matRotX[9] = {1, 0, 0, 0, cTauX, sTauX, 0, -sTauX, cTauX};
+    const double matRotY[9] = {cTauY, 0, -sTauY, 0, 1, 0, sTauY, 0, cTauY};
+    double R[9];
+    matx33_mul(matRotY, matRotX, R);
+    const double matProjZ[9] = {R[8], 0, -R[2], 0, R[8], -R[5], 0, 0, 1};
+    matx33_mul(matProjZ, R, matTilt);
+    const double inv = 1. / R[8];
+    const double invMatProjZ[9] = {inv, 0, inv * R[2], 0, inv, inv * R[5], 0, 0, 1};
+    const double Rt[9] = {R[0], R[3], R[6], R[1], R[4], R[7], R[2], R[5], R[8]};
+    matx33_mul(Rt, invMatProjZ, invMatTilt);
+}
+// the lens of an OpenCV distortion vector of n = 4, 5, 8, 12 or 14 entries, zero-padded to 14.  False (L untouched) for another
+// n, a non-finite coefficient, or |tau_x| or |tau_y| >= pi/2, where 1 / matRotXY(2, 2) is no longer a finite tilt.
+inline bool make_lens_full(const double* coeffs, int n, LensFull& L) {
+    if (!coeffs || !(n == 4 || n == 5 || n == 8 || n == 12 || n == 14)) return false;
+    double k[14] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+    for (int i = 0; i < n; i++) {
+        if (!(coeffs[i] - coeffs[i] == 0.0)) return false;
+        k[i] = coeffs[i];
+    }
+    if (!(fabs(k[12]) < kHalfPi && fabs(k[13]) < kHalfPi)) return false;
+    for (int i = 0; i < 14; i++) L.k[i] = k[i];
+    tilt_matrices(k[12], k[13], L.tilt, L.itilt);
+    return true;
 }
 
 // ------------------------------------------------------------------------------------------------ equidistant fisheye
@@ -99,8 +168,6 @@ ALVA_CAM_FN void project_dist(const double* K4, const double* D4, const double* 
 // glibc and CUDA's libdevice round them differently, so one plain-arithmetic version keeps the device, the state machine and
 // the CPU test backend bit-identical.  Against OpenCV (glibc) they agree to the last double bit on nearly every point; a float
 // result can only differ when the double lies within a few ulps of a float rounding boundary (tests/test_oracle_fisheye.py).
-
-constexpr double kHalfPi = 1.57079632679489661923;   // CV_PI / 2.
 
 // the high half of x with the low 32 bits cleared
 ALVA_CAM_FN double hi_word(double x) {
@@ -278,16 +345,17 @@ ALVA_CAM_FN void project_pinhole(const double* K4, const double* p, float* out) 
 
 // A rotation-compensated KLT prior (System's gyro mode, not in the reference): the bearing bv of a previous-frame keypoint
 // turned into the current camera, c = R^T bv (R = the camera's rotation from the previous frame to the current one, row-major),
-// and projected through the lens (0 pinhole, 1 radial-tangential, 2 fisheye; D4 unused for the pinhole) -- the infinite
-// homography, exact for a pure rotation.  Returns true and writes out[2] only when the ray is in front of the camera (z > 0)
+// and projected through the lens (0 pinhole, 1 radial-tangential, 2 fisheye, 3 the full OpenCV vector F; D4 unused for the
+// pinhole and lens 3, F only for lens 3) -- the infinite homography, exact for a pure rotation.  Returns true and writes out[2] only when the ray is in front of the camera (z > 0)
 // and its projection lies inside the w x h image (Camera::inImage); otherwise out is left as it was.
 ALVA_CAM_FN bool rotate_prior(int lens, const double* K4, const double* D4, int w, int h, const double* R9, const double* bv,
-                              float* out) {
+                              float* out, const LensFull* F = nullptr) {
     double c[3];
     for (int i = 0; i < 3; i++) c[i] = (R9[i] * bv[0] + R9[3 + i] * bv[1]) + R9[6 + i] * bv[2];
     if (!(c[2] > 0.0)) return false;
     float o[2];
-    if (lens == 2) project_dist_fisheye(K4, D4, c, o);
+    if (lens == 3) project_dist_full(K4, F->k, F->tilt, c, o);
+    else if (lens == 2) project_dist_fisheye(K4, D4, c, o);
     else if (lens == 1) project_dist(K4, D4, c, o);
     else project_pinhole(K4, c, o);
     if (!(o[0] >= 0 && o[1] >= 0 && o[0] < w && o[1] < h)) return false;

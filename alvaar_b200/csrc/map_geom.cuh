@@ -10,8 +10,9 @@
 
 namespace alva_geom {
 
-// LENS_NONE: the zero-distortion projection; LENS_RADTAN / LENS_FISHEYE: the lens models of camera_model.h (Camera::Lens values)
-enum { LENS_NONE = 0, LENS_RADTAN = 1, LENS_FISHEYE = 2 };
+// LENS_NONE: the zero-distortion projection; LENS_RADTAN / LENS_FISHEYE / LENS_FULL: the lens models of camera_model.h
+// (Camera::Lens values; LENS_FULL is OpenCV's 14-coefficient vector with its tilt)
+enum { LENS_NONE = 0, LENS_RADTAN = 1, LENS_FISHEYE = 2, LENS_FULL = 3 };
 
 __device__ __forceinline__ void quat_R(const double* q, double* R) {
     const double n = sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
@@ -31,10 +32,13 @@ __device__ __forceinline__ void world_to_cam(const double* Twc, const double* X,
 #pragma unroll
     for (int i = 0; i < 3; i++) c[i] = (R[i] * X[0] + R[3 + i] * X[1] + R[6 + i] * X[2]) + ti[i];
 }
-// K4 = {fx, fy, cx, cy}; D4: the lens coefficients (unused for LENS_NONE)
+// K4 = {fx, fy, cx, cy}; D4: the lens coefficients (unused for LENS_NONE and LENS_FULL); F: the LENS_FULL lens (only there)
 template <int LENS>
-__device__ __forceinline__ void project_cam(const double* K4, const double* D4, const double* c, float* px) {
-    if constexpr (LENS == LENS_RADTAN) {
+__device__ __forceinline__ void project_cam(const double* K4, const double* D4, const double* c, float* px,
+                                            const alva_cam::LensFull* F = nullptr) {
+    if constexpr (LENS == LENS_FULL) {
+        alva_cam::project_dist_full(K4, F->k, F->tilt, c, px);
+    } else if constexpr (LENS == LENS_RADTAN) {
         alva_cam::project_dist(K4, D4, c, px);
     } else if constexpr (LENS == LENS_FISHEYE) {
         alva_cam::project_dist_fisheye(K4, D4, c, px);

@@ -6,7 +6,7 @@
 //   MapPoint::computeMinDescDist           src/slam/src/map_point.cpp:204-222  (cv::norm(NORM_HAMMING), all pairs)
 //   Frame::getSurroundingKeypoints         src/slam/src/frame.cpp:313-341
 //   CameraCalibration::projectCamToImageDist  src/slam/src/camera_calibration.cpp:34-55  (with distortion: camera_model.h,
-//                                             radial-tangential or equidistant fisheye)
+//                                             radial-tangential, its full 14-coefficient form, or equidistant fisheye)
 //
 // How: the reference walks hash maps (map point -> shared_ptr -> per-keyframe descriptor map -> cv::Mat) once per candidate.
 // Here the map lives in flat SoA arenas in HBM (world points, CSR observation lists, CSR descriptor lists) and one warp
@@ -54,15 +54,21 @@ struct MatchParams {
     int32_t* n_match;
     double dist[4];   // k1 k2 p1 p2 (LENS_RADTAN) or k1 k2 k3 k4 (LENS_FISHEYE)
 };
+// LENS_FULL's parameters: the same, and the 14 coefficients with their tilt matrices (the other lenses keep MatchParams)
+struct MatchParamsFull : MatchParams { alva_cam::LensFull L; };
+template <int LENS> struct MatchArgs { using type = MatchParams; };
+template <> struct MatchArgs<alva_geom::LENS_FULL> { using type = MatchParamsFull; };
 
 using alva_geom::world_to_cam;
 using alva_geom::LENS_NONE;
 using alva_geom::LENS_RADTAN;
 using alva_geom::LENS_FISHEYE;
+using alva_geom::LENS_FULL;
 template <int LENS>
-__device__ __forceinline__ void project_cam(const MatchParams& P, const double* c, float* px) {
+__device__ __forceinline__ void project_cam(const typename MatchArgs<LENS>::type& P, const double* c, float* px) {
     const double K4[4] = {P.fx, P.fy, P.cx, P.cy};
-    alva_geom::project_cam<LENS>(K4, P.dist, c, px);
+    if constexpr (LENS == LENS_FULL) alva_geom::project_cam<LENS>(K4, nullptr, c, px, &P.L);
+    else alva_geom::project_cam<LENS>(K4, P.dist, c, px);
 }
 
 // one CTA: observed flags, the frame's grid (cell -> keypoints in insertion order), per-keypoint result keys
@@ -108,7 +114,7 @@ __global__ void __launch_bounds__(1024) match_prepare_kernel(const MatchParams P
 }
 
 template <int LENS>
-__global__ void __launch_bounds__(128) match_local_kernel(const MatchParams P) {
+__global__ void __launch_bounds__(128) match_local_kernel(const typename MatchArgs<LENS>::type P) {
     const int lane = threadIdx.x & 31;
     const int li = (int)((blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5);
     if (li >= P.n_local) return;
@@ -213,13 +219,14 @@ __global__ void match_finalize_kernel(const MatchParams P) {
     atomicAdd(P.n_match, 1);
 }
 
-// lens: LENS_NONE (coef4 unused), LENS_RADTAN or LENS_FISHEYE with its four coefficients (checked by the caller)
+// lens: LENS_NONE (coef4 unused), LENS_RADTAN or LENS_FISHEYE with its four coefficients, or LENS_FULL with F (checked by the
+// caller)
 int match_to_map_launch(alva_ctx* ctx, int w, int h, int cell, double fx, double fy, double cx, double cy, const double* Twc_cur,
                         int n_kp, const int32_t* kp_mp, const float* kp_px, int nkp3d, int n_kf, const double* kf_Twc, int n_mp,
                         const double* mp_wpt, const uint8_t* mp_is3d, const int32_t* obs_start, const int32_t* obs_kf,
                         const float* obs_px, const int32_t* desc_start, const uint8_t* desc, int n_local, const int32_t* local_mp,
                         float max_proj_err, float dist_ratio, int32_t* kp_match, float* kp_dist, int32_t* n_match, int lens,
-                        const double* coef4) {
+                        const double* coef4, const alva_cam::LensFull* F = nullptr) {
     if (!ctx || !Twc_cur || !kp_mp || !kp_px || !kf_Twc || !mp_wpt || !mp_is3d || !obs_start || !obs_kf || !obs_px || !desc_start ||
         !desc || !local_mp || !kp_match || !n_match || n_kp < 1 || n_mp < 1 || n_local < 1 || cell < 1) {
         alva_set_error("alva_k_match_to_map: bad argument");
@@ -227,8 +234,10 @@ int match_to_map_launch(alva_ctx* ctx, int w, int h, int cell, double fx, double
     }
     if (n_kf > 64) { alva_set_error("alva_k_match_to_map: at most 64 keyframes (the reference's window is 30), got %d", n_kf); return ALVA_E_INVALID; }
     if (((uintptr_t)desc & 15) != 0) { alva_set_error("alva_k_match_to_map: desc must be 16-byte aligned"); return ALVA_E_INVALID; }
-    MatchParams P{};
-    if (lens != LENS_NONE) for (int i = 0; i < 4; i++) P.dist[i] = coef4[i];
+    MatchParamsFull PF{};
+    MatchParams& P = PF;
+    if (lens == LENS_FULL) PF.L = *F;
+    else if (lens != LENS_NONE) for (int i = 0; i < 4; i++) P.dist[i] = coef4[i];
     P.w = w; P.h = h; P.cell = cell;
     P.ncw = (int)ceilf((float)w / (float)cell); P.nch = (int)ceilf((float)h / (float)cell);   // frame.cpp:14-15
     P.fx = fx; P.fy = fy; P.cx = cx; P.cy = cy;
@@ -251,7 +260,8 @@ int match_to_map_launch(alva_ctx* ctx, int w, int h, int cell, double fx, double
     P.kp_match = kp_match; P.kp_dist = kp_dist; P.n_match = n_match;
     match_prepare_kernel<<<1, 1024, 0, ctx->stream>>>(P);
     ALVA_LAUNCH_CHECK(ctx);
-    if (lens == LENS_RADTAN) match_local_kernel<LENS_RADTAN><<<(n_local * 32 + 127) / 128, 128, 0, ctx->stream>>>(P);
+    if (lens == LENS_FULL) match_local_kernel<LENS_FULL><<<(n_local * 32 + 127) / 128, 128, 0, ctx->stream>>>(PF);
+    else if (lens == LENS_RADTAN) match_local_kernel<LENS_RADTAN><<<(n_local * 32 + 127) / 128, 128, 0, ctx->stream>>>(P);
     else if (lens == LENS_FISHEYE) match_local_kernel<LENS_FISHEYE><<<(n_local * 32 + 127) / 128, 128, 0, ctx->stream>>>(P);
     else match_local_kernel<LENS_NONE><<<(n_local * 32 + 127) / 128, 128, 0, ctx->stream>>>(P);
     ALVA_LAUNCH_CHECK(ctx);
@@ -291,6 +301,22 @@ extern "C" int alva_k_match_to_map_fisheye(alva_ctx* ctx, int w, int h, int cell
     return match_to_map_launch(ctx, w, h, cell, fx, fy, cx, cy, Twc_cur, n_kp, kp_mp, kp_px, nkp3d, n_kf, kf_Twc, n_mp, mp_wpt, mp_is3d,
                                obs_start, obs_kf, obs_px, desc_start, desc, n_local, local_mp, max_proj_err, dist_ratio, kp_match, kp_dist,
                                n_match, LENS_FISHEYE, fisheye4);
+}
+
+extern "C" int alva_k_match_to_map_full(alva_ctx* ctx, int w, int h, int cell, double fx, double fy, double cx, double cy,
+                                        const double* Twc_cur, int n_kp, const int32_t* kp_mp, const float* kp_px, int nkp3d, int n_kf,
+                                        const double* kf_Twc, int n_mp, const double* mp_wpt, const uint8_t* mp_is3d,
+                                        const int32_t* obs_start, const int32_t* obs_kf, const float* obs_px, const int32_t* desc_start,
+                                        const uint8_t* desc, int n_local, const int32_t* local_mp, float max_proj_err, float dist_ratio,
+                                        int32_t* kp_match, float* kp_dist, int32_t* n_match, const double* coeffs, int ncoeffs) { AlvaDeviceGuard guard__(ctx);
+    alva_cam::LensFull L;
+    if (!alva_cam::make_lens_full(coeffs, ncoeffs, L)) {
+        alva_set_error("alva_k_match_to_map_full: coeffs must hold 4, 5, 8, 12 or 14 finite values with |tau_x|, |tau_y| < pi/2");
+        return ALVA_E_INVALID;
+    }
+    return match_to_map_launch(ctx, w, h, cell, fx, fy, cx, cy, Twc_cur, n_kp, kp_mp, kp_px, nkp3d, n_kf, kf_Twc, n_mp, mp_wpt, mp_is3d,
+                               obs_start, obs_kf, obs_px, desc_start, desc, n_local, local_mp, max_proj_err, dist_ratio, kp_match, kp_dist,
+                               n_match, LENS_FULL, nullptr, &L);
 }
 
 extern "C" int alva_k_match_to_map(alva_ctx* ctx, int w, int h, int cell, double fx, double fy, double cx, double cy,

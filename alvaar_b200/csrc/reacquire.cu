@@ -50,6 +50,10 @@ struct ReacqParams {
     int32_t* q_row;
     int32_t* q_dist;
 };
+// LENS_FULL's parameters: the same, and the 14 coefficients with their tilt matrices (the other lenses keep ReacqParams)
+struct ReacqParamsFull : ReacqParams { alva_cam::LensFull L; };
+template <int LENS> struct ReacqArgs { using type = ReacqParams; };
+template <> struct ReacqArgs<alva_geom::LENS_FULL> { using type = ReacqParamsFull; };
 
 __device__ __forceinline__ int clampi(int v, int lo, int hi) { return v < lo ? lo : (v > hi ? hi : v); }
 
@@ -99,7 +103,7 @@ __global__ void __launch_bounds__(1024) reacq_grid_kernel(const ReacqParams P) {
 }
 
 template <int LENS>
-__global__ void __launch_bounds__(128) reacq_match_kernel(const ReacqParams P) {
+__global__ void __launch_bounds__(128) reacq_match_kernel(const typename ReacqArgs<LENS>::type P) {
     const int m = blockIdx.x * blockDim.x + threadIdx.x;
     if (m >= P.n_mp) return;
     if (P.skip && P.skip[m]) return;
@@ -112,7 +116,8 @@ __global__ void __launch_bounds__(128) reacq_match_kernel(const ReacqParams P) {
     const float view_angle = (float)(c[2] / sqrt(c[0] * c[0] + c[1] * c[1] + c[2] * c[2]));
     if (fabs((double)view_angle) < (double)P.view_th) return;                          // :432
     float proj[2];
-    alva_geom::project_cam<LENS>(P.K4, P.D4, c, proj);
+    if constexpr (LENS == alva_geom::LENS_FULL) alva_geom::project_cam<LENS>(P.K4, nullptr, c, proj, &P.L);
+    else alva_geom::project_cam<LENS>(P.K4, P.D4, c, proj);
     if (!(proj[0] >= 0 && proj[1] >= 0 && (double)proj[0] < (double)P.w && (double)proj[1] < (double)P.h)) return;
     const float r = P.radius;
     const int cx0 = max(0, (int)floorf((proj[0] - r - 1.f) / (float)P.cell)), cx1 = min(P.ncw - 1, (int)floorf((proj[0] + r + 1.f) / (float)P.cell));
@@ -166,27 +171,35 @@ extern "C" int alva_k_match_frame_to_map(alva_ctx* ctx, int w, int h, int cell, 
                                          const double* coef4, const double* Twc, int n_mp, const double* wpt, const int32_t* desc_start,
                                          const uint8_t* desc, const uint8_t* skip, int nq, const float* q_px, const uint8_t* q_desc,
                                          const uint8_t* q_kept, float radius, int32_t* q_row, int32_t* q_dist) { AlvaDeviceGuard guard__(ctx);
-    if (!ctx || !Twc || n_mp < 0 || nq < 0 || w < 1 || h < 1 || cell < 1 || lens < alva_geom::LENS_NONE || lens > alva_geom::LENS_FISHEYE ||
+    if (!ctx || !Twc || n_mp < 0 || nq < 0 || w < 1 || h < 1 || cell < 1 || lens < alva_geom::LENS_NONE || lens > alva_geom::LENS_FULL ||
         (n_mp > 0 && (!wpt || !desc_start || !desc)) || (nq > 0 && (!q_px || !q_desc || !q_kept || !q_row || !q_dist)) ||
         !(radius >= 0.f) || !(fx > 0) || !(fy > 0)) {
         alva_set_error("alva_k_match_frame_to_map: bad argument");
         return ALVA_E_INVALID;
     }
+    ReacqParamsFull PF{};
+    ReacqParams& P = PF;
     if (lens != alva_geom::LENS_NONE) {
         if (!coef4) { alva_set_error("alva_k_match_frame_to_map: coef4 is required with a lens"); return ALVA_E_INVALID; }
-        for (int i = 0; i < 4; i++)
-            if (!isfinite(coef4[i])) { alva_set_error("alva_k_match_frame_to_map: non-finite lens coefficient"); return ALVA_E_INVALID; }
+        if (lens == alva_geom::LENS_FULL) {   // 14 coefficients
+            if (!alva_cam::make_lens_full(coef4, 14, PF.L)) {
+                alva_set_error("alva_k_match_frame_to_map: lens 3 needs 14 finite coefficients with |tau_x|, |tau_y| < pi/2");
+                return ALVA_E_INVALID;
+            }
+        } else {
+            for (int i = 0; i < 4; i++)
+                if (!isfinite(coef4[i])) { alva_set_error("alva_k_match_frame_to_map: non-finite lens coefficient"); return ALVA_E_INVALID; }
+        }
     }
     if ((n_mp > 0 && ((uintptr_t)desc & 15) != 0) || (nq > 0 && ((uintptr_t)q_desc & 15) != 0)) {
         alva_set_error("alva_k_match_frame_to_map: desc and q_desc must be 16-byte aligned");
         return ALVA_E_INVALID;
     }
     if (nq == 0) return 0;
-    ReacqParams P{};
     P.w = w; P.h = h; P.cell = cell;
     P.ncw = (int)ceilf((float)w / (float)cell); P.nch = (int)ceilf((float)h / (float)cell);   // frame.cpp:14-15
     P.K4[0] = fx; P.K4[1] = fy; P.K4[2] = cx; P.K4[3] = cy;
-    if (lens != alva_geom::LENS_NONE) for (int i = 0; i < 4; i++) P.D4[i] = coef4[i];
+    if (lens == alva_geom::LENS_RADTAN || lens == alva_geom::LENS_FISHEYE) for (int i = 0; i < 4; i++) P.D4[i] = coef4[i];
     P.Twc = Twc; P.n_mp = n_mp; P.wpt = wpt; P.desc_start = desc_start; P.desc = desc; P.skip = skip;
     P.nq = nq; P.q_px = q_px; P.q_desc = q_desc; P.q_kept = q_kept;
     // mapper.cpp:365-385, 436: the thresholds in the reference's float arithmetic (on the host, as match.cu)
@@ -206,7 +219,8 @@ extern "C" int alva_k_match_frame_to_map(alva_ctx* ctx, int w, int h, int cell, 
     ALVA_LAUNCH_CHECK(ctx);
     if (n_mp > 0) {
         const int nb = (n_mp + 127) / 128;
-        if (lens == alva_geom::LENS_RADTAN) reacq_match_kernel<alva_geom::LENS_RADTAN><<<nb, 128, 0, ctx->stream>>>(P);
+        if (lens == alva_geom::LENS_FULL) reacq_match_kernel<alva_geom::LENS_FULL><<<nb, 128, 0, ctx->stream>>>(PF);
+        else if (lens == alva_geom::LENS_RADTAN) reacq_match_kernel<alva_geom::LENS_RADTAN><<<nb, 128, 0, ctx->stream>>>(P);
         else if (lens == alva_geom::LENS_FISHEYE) reacq_match_kernel<alva_geom::LENS_FISHEYE><<<nb, 128, 0, ctx->stream>>>(P);
         else reacq_match_kernel<alva_geom::LENS_NONE><<<nb, 128, 0, ctx->stream>>>(P);
         ALVA_LAUNCH_CHECK(ctx);

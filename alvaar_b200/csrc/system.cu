@@ -29,8 +29,9 @@
 //                (not in the reference: alva_system_set_gyro)
 // There is no CPU fallback: configure() fails without an sm_90 (H100) device.  Lens distortion: the JS shim always passes zeros
 // (system.js:84-141) and configure() rejects non-zero coefficients; setDistortion() (alva_system_set_distortion) sets them on a
-// configured System, and setFisheye() (alva_system_set_fisheye) selects OpenCV's equidistant fisheye model instead.  With a
-// lens on, klt and detect undistort the points they return with alva_k_undistort_points (or its fisheye twin) on the device, in
+// configured System, setFisheye() (alva_system_set_fisheye) selects OpenCV's equidistant fisheye model instead, and
+// setDistortionCoeffs() (alva_system_set_distortion_coeffs) takes OpenCV's whole 5- to 14-entry vector.  With a lens on, klt and
+// detect undistort the points they return with alva_k_undistort_points (or its fisheye or full-vector twin) on the device, in
 // the same download (camera.cu, camera_model.h).
 #include "alva_common.cuh"
 #include "../../include/alva_b200.h"
@@ -48,8 +49,10 @@ int alva_undistort_points_launch(alva_ctx* ctx, const float* px, const int32_t* 
                                  const double* D4, float* unpx);
 int alva_undistort_points_fisheye_launch(alva_ctx* ctx, const float* px, const int32_t* counts, int nframes, int cap, const double* K4,
                                          const double* D4, float* unpx);
+int alva_undistort_points_full_launch(alva_ctx* ctx, const float* px, const int32_t* counts, int nframes, int cap, const double* K4,
+                                      const alva_cam::LensFull& L, float* unpx);
 int alva_rotate_priors_launch(alva_ctx* ctx, const double* bv, const uint8_t* flag, int n, int w, int h, const double* K4, const double* D4,
-                              int lens, const double* R9, float* prior, uint8_t* rotated);
+                              int lens, const double* R9, float* prior, uint8_t* rotated, const alva_cam::LensFull* F);
 int alva_pose_chain_launch(alva_ctx* ctx, int n, int cap, const double* bvs, const double* X, const double* uv, const double* K4,
                            float fx, float fy, uint32_t seed, double* T12, double* info, uint8_t* o1, double* uv2, double* X2,
                            int32_t* n2, double* pose7, uint8_t* o2, double* summ, double huber, double chi2);
@@ -140,9 +143,11 @@ struct CudaBackend {
     size_t clahe_lut_bytes = 0;
     cudaGraphExec_t clahe_graph[2] = {nullptr, nullptr};
     // lens distortion (CameraCalibration::D_): when on, klt() and detect() also return the undistorted positions of their points
-    // (unpx()); with it off nothing here is allocated or launched.  fisheye: through the equidistant fisheye model.
-    bool has_dist = false, fisheye = false;
+    // (unpx()); with it off nothing here is allocated or launched.  fisheye: through the equidistant fisheye model; full:
+    // through OpenCV's 14-coefficient model LF (lens 3).
+    bool has_dist = false, fisheye = false, full = false;
     double K4[4] = {0, 0, 0, 0}, D4[4] = {0, 0, 0, 0};
+    alva_cam::LensFull LF{};
     float* unpx_dev = nullptr;
     std::vector<float> unpx_host;
 
@@ -224,7 +229,7 @@ struct CudaBackend {
         for (void** b : rbufs) if (*b) { cudaFree(*b); *b = nullptr; }
         reloc_tab_bytes = 0; reloc_ws_cap = 0; reloc_loaded = false;
         rq.release();
-        has_dist = fisheye = false;
+        has_dist = fisheye = full = false;
         cap = cap_alloc = 0;
         cell = 40;
         clahe = false;
@@ -257,7 +262,7 @@ struct CudaBackend {
 
     int set_distortion(const double* d) {
         has_dist = d[0] != 0.0 || d[1] != 0.0 || d[2] != 0.0 || d[3] != 0.0;
-        fisheye = false;
+        fisheye = full = false;
         for (int i = 0; i < 4; i++) D4[i] = d[i];
         K4[0] = fx; K4[1] = fy; K4[2] = cx; K4[3] = cy;
         if (has_dist && !unpx_dev) SYS_CUDA(cudaMalloc(&unpx_dev, (size_t)cap_alloc * 8));
@@ -265,13 +270,26 @@ struct CudaBackend {
     }
     int set_fisheye(bool on, const double* k) {
         has_dist = fisheye = on;
+        full = false;
         for (int i = 0; i < 4; i++) D4[i] = on ? k[i] : 0.0;
         K4[0] = fx; K4[1] = fy; K4[2] = cx; K4[3] = cy;
         if (has_dist && !unpx_dev) SYS_CUDA(cudaMalloc(&unpx_dev, (size_t)cap_alloc * 8));
         return 0;
     }
+    // lens 3 (Camera::FULL, already built by the state machine's camera)
+    int set_full(const alva_cam::LensFull& L) {
+        has_dist = full = true;
+        fisheye = false;
+        LF = L;
+        for (int i = 0; i < 4; i++) D4[i] = L.k[i];
+        K4[0] = fx; K4[1] = fy; K4[2] = cx; K4[3] = cy;
+        if (!unpx_dev) SYS_CUDA(cudaMalloc(&unpx_dev, (size_t)cap_alloc * 8));
+        return 0;
+    }
+    int lens_id() const { return full ? 3 : (fisheye ? 2 : (has_dist ? 1 : 0)); }
     // Frame::computeKeypoint's undistortImagePoint of the given points, through the lens model that is on
     int undistort_launch(const float* px, const int32_t* counts, int n, float* unpx) {
+        if (full) return alva_undistort_points_full_launch(ctx, px, counts, 1, n, K4, LF, unpx);
         return fisheye ? alva_undistort_points_fisheye_launch(ctx, px, counts, 1, n, K4, D4, unpx)
                        : alva_undistort_points_launch(ctx, px, counts, 1, n, K4, D4, unpx);
     }
@@ -428,7 +446,7 @@ struct CudaBackend {
         SYS_CUDA(cudaMemcpyAsync(stg.d, stg.h, up_end, cudaMemcpyHostToDevice, st));
         if (bv) {
             const double K[4] = {fx, fy, cx, cy};
-            if (int e = alva_rotate_priors_launch(ctx, db, df, n, w, h, K, D4, fisheye ? 2 : (has_dist ? 1 : 0), dR9, dq, dr)) return e;
+            if (int e = alva_rotate_priors_launch(ctx, db, df, n, w, h, K, D4, lens_id(), dR9, dq, dr, &LF)) return e;
         }
         const int prev = cur ^ 1;
         if (int e = alva_k_klt_fb(ctx, img[prev], der[prev], img[cur], der[cur], w, h, 1, nlev - 1, levels, 9, 30.0f, 0.5f, dp, dq, nullptr, n, dg))
@@ -676,8 +694,7 @@ struct CudaBackend {
         memcpy(hT, Twc7, 56); memcpy(hp, qpx, (size_t)nq * 8); memcpy(hd, qdesc, (size_t)nq * 32); memcpy(hk, qkept, nq); memcpy(hs, skip, n_grp);
         SYS_CUDA(cudaMemcpyAsync(rq.d, rq.h, up_end, cudaMemcpyHostToDevice, st));
         const size_t ds_b = al256((size_t)(n_grp + 1) * 4), w_b = al256((size_t)n_grp * 24);   // upload_table's layout
-        const int lens = fisheye ? 2 : (has_dist ? 1 : 0);
-        if (int e = alva_k_match_frame_to_map(ctx, w, h, cell, fx, fy, cx, cy, lens, D4, dT, n_grp, (const double*)(reloc_tab + ds_b),
+        if (int e = alva_k_match_frame_to_map(ctx, w, h, cell, fx, fy, cx, cy, lens_id(), full ? LF.k : D4, dT, n_grp, (const double*)(reloc_tab + ds_b),
                                               (const int32_t*)reloc_tab, reloc_tab + ds_b + w_b, ds, nq, dp, dd, dk, radius, dr, ddist))
             return e;
         SYS_CUDA(cudaMemcpyAsync(rq.h + down_off, rq.d + down_off, down_end - down_off, cudaMemcpyDeviceToHost, st));
@@ -766,7 +783,11 @@ struct CudaBackend {
         int32_t* lm = arena_put(m.local_mp.data(), n_local);
         int32_t* out = arena_take<int32_t>(n_kp);
         int32_t* nm = arena_take<int32_t>(4);
-        if (m.fisheye) {
+        if (m.full) {
+            if (int e = alva_k_match_to_map_full(ctx, w, h, cell, fx, fy, cx, cy, Tc, (int)n_kp, kpmp, kppx, m.nkp3d, (int)(n_kf ? n_kf : 1), kfT,
+                                                 (int)n_mp, wpt, is3, os, ok, op, ds, dd, (int)n_local, lm, 2.0f, 0.2f, out, nullptr, nm, m.lf.k, 14))
+                return e;
+        } else if (m.fisheye) {
             if (int e = alva_k_match_to_map_fisheye(ctx, w, h, cell, fx, fy, cx, cy, Tc, (int)n_kp, kpmp, kppx, m.nkp3d, (int)(n_kf ? n_kf : 1), kfT,
                                                     (int)n_mp, wpt, is3, os, ok, op, ds, dd, (int)n_local, lm, 2.0f, 0.2f, out, nullptr, nm, m.dist))
                 return e;
@@ -845,6 +866,20 @@ public:
             if (!std::isfinite(v)) { alva_set_error("alva_system_set_fisheye: non-finite coefficient"); return ALVA_E_INVALID; }
         if (int e = be_.set_fisheye(enabled != 0, k)) return e;
         core_.setFisheye(enabled != 0, k);
+        return 0;
+    }
+    // OpenCV's distortion vector of n = 4, 5, 8, 12 or 14 entries (cv::calibrateCamera's output): the pinhole when all are zero,
+    // exactly setDistortion when only k1 k2 p1 p2 are, else the full model on every lens path.  Like setDistortion, the tracker
+    // and the map restart and configure() clears it; it replaces, and is replaced by, setDistortion and setFisheye.
+    int setDistortionCoeffs(const double* coeffs, int n) {
+        if (!configured_) { alva_set_error("System: not configured"); return ALVA_E_STATE; }
+        alva_sys::Camera c = core_.cam;
+        if (!c.setDistortionCoeffs(coeffs, n)) {
+            alva_set_error("alva_system_set_distortion_coeffs: need 4, 5, 8, 12 or 14 finite coefficients with |tau_x|, |tau_y| < pi/2 (n = %d)", n);
+            return ALVA_E_INVALID;
+        }
+        if (int e = c.lens == alva_sys::Camera::FULL ? be_.set_full(c.full) : be_.set_distortion(c.dist)) return e;
+        core_.setDistortionCoeffs(coeffs, n);
         return 0;
     }
     int lensDrops() const { return core_.n_lens_drops; }
@@ -1094,6 +1129,10 @@ extern "C" int alva_system_set_distortion(alva_system* s, double k1, double k2, 
 extern "C" int alva_system_set_fisheye(alva_system* s, int enabled, double k1, double k2, double k3, double k4) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
     if (!s) { alva_set_error("alva_system_set_fisheye: null handle"); return ALVA_E_INVALID; }
     return s->sys.setFisheye(enabled, k1, k2, k3, k4);
+}
+extern "C" int alva_system_set_distortion_coeffs(alva_system* s, const double* coeffs, int n) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);
+    if (!s) { alva_set_error("alva_system_set_distortion_coeffs: null handle"); return ALVA_E_INVALID; }
+    return s->sys.setDistortionCoeffs(coeffs, n);
 }
 extern "C" int alva_system_lens_drops(alva_system* s) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1); return s ? s->sys.lensDrops() : ALVA_E_INVALID; }
 extern "C" int alva_system_set_preset(alva_system* s, int preset) { AlvaDeviceGuard guard__(s ? s->sys.device_ : -1);

@@ -153,10 +153,12 @@ struct Camera {
     // equidistant fisheye model (k1 k2 k3 k4 on theta).  has_dist = a model other than the pinhole is applied.  The
     // radial-tangential model with all coefficients zero is the pinhole: the two functions that apply it below then take their
     // pinhole forms, which give the same bits.  A fisheye lens with zero coefficients is the equidistant projection, not the
-    // pinhole, so the model is never inferred from the coefficients.
-    enum Lens { PINHOLE = 0, RADTAN = 1, FISHEYE = 2 };
+    // pinhole, so the model is never inferred from the coefficients.  FULL: OpenCV's whole distortion vector (k3, the rational,
+    // thin-prism and tilted models; full.k, dist = its first four), chosen only when an entry past p2 is non-zero.
+    enum Lens { PINHOLE = 0, RADTAN = 1, FISHEYE = 2, FULL = 3 };
     int lens = PINHOLE;
     double dist[4] = {0, 0, 0, 0};
+    alva_cam::LensFull full{};
     bool has_dist = false;
     void setDistortion(const double* d) {
         has_dist = false;
@@ -167,6 +169,20 @@ struct Camera {
         for (int i = 0; i < 4; i++) dist[i] = on ? k[i] : 0.0;
         lens = on ? FISHEYE : PINHOLE;
         has_dist = on;
+    }
+    // an OpenCV distortion vector of n = 4, 5, 8, 12 or 14 entries: all zero -> the pinhole, only k1 k2 p1 p2 non-zero -> RADTAN
+    // (exactly setDistortion), anything else -> FULL.  False, and nothing changed, for a vector alva_cam::make_lens_full refuses.
+    bool setDistortionCoeffs(const double* c, int n) {
+        alva_cam::LensFull L;
+        if (!alva_cam::make_lens_full(c, n, L)) return false;
+        bool rest = false;
+        for (int i = 4; i < 14; i++) rest = rest || L.k[i] != 0.0;
+        if (!rest) { setDistortion(L.k); return true; }
+        full = L;
+        for (int i = 0; i < 4; i++) dist[i] = L.k[i];
+        lens = FULL;
+        has_dist = true;
+        return true;
     }
     // the value cv::fisheye::undistortPoints returns for a pixel it cannot undistort (Newton did not converge, or theta flipped):
     // 1e6 px outside any image, never the result of the radial-tangential model or of a converged fisheye point in practice
@@ -181,6 +197,14 @@ struct Camera {
         k00 = fy * id; k02 = (-(cx * fy)) * id; k11 = fx * id; k12 = (-(fx * cy)) * id; k22 = (fx * fy) * id;
     }
     void undistort(float u, float v, float& ux, float& uy) const {
+        if (lens == FULL) {
+            double k[4];
+            float o[2];
+            K4(k);
+            alva_cam::undistort_point_full(k, full.k, full.itilt, u, v, o);
+            ux = o[0]; uy = o[1];
+            return;
+        }
         if (lens == FISHEYE) {
             double k[4];
             float o[2];
@@ -220,6 +244,14 @@ struct Camera {
         u = (float)(fx * (p[0] * iz) + cx); v = (float)(fy * (p[1] * iz) + cy);
     }
     void projCamToImageDist(const double* p, float& u, float& v) const {   // :34-55: cv::projectPoints on a FLOAT point
+        if (lens == FULL) {
+            double k[4];
+            float o[2];
+            K4(k);
+            alva_cam::project_dist_full(k, full.k, full.tilt, p, o);
+            u = o[0]; v = o[1];
+            return;
+        }
         if (lens == FISHEYE) {
             double k[4];
             float o[2];
@@ -517,6 +549,8 @@ struct MatchProblem {   // Mapper::matchToMap on flat arrays (the contract of al
     bool has_dist = false;              // lens distortion of the projections (Camera::dist)
     bool fisheye = false;               // ... through the equidistant fisheye model instead of the radial-tangential one
     double dist[4] = {0, 0, 0, 0};
+    bool full = false;                  // ... through OpenCV's 14-coefficient model (lf; dist = its first four)
+    alva_cam::LensFull lf{};
 };
 // the map a lost frame is matched against: every map point that is 3-D and has a descriptor, in ascending id order; its
 // keyframe descriptors (MapPoint::kfdesc) in ascending keyframe id order, CSR.  The map is frozen while lost: built once, when
@@ -651,7 +685,8 @@ public:
     // setGyro needs a backend with klt_rotated (MAP_STATE otherwise).  R_ci (NULL: identity) takes IMU-axis vectors to camera
     // axes; bias (NULL: zero) is a constant gyro bias in rad/s on the IMU axes.  A non-finite value, or an R_ci with an entry
     // of R^T R - I above 1e-9 or a negative determinant, is refused (MAP_INVALID).  Disabling drops the samples.  configure
-    // ends the mode; reset, setPreset, setDistortion, setFisheye, setRelocalisation, setLocalisationOnly and loadMap keep it.
+    // ends the mode; reset, setPreset, setDistortion, setFisheye, setDistortionCoeffs, setRelocalisation, setLocalisationOnly and
+    // loadMap keep it.
     int setGyro(bool on, const double* Rci, const double* bias) {
         if (!on) { gyro_on = gyro_ok = false; gyro_buf.clear(); gyroIdentity(gyro_dRc); return 0; }
         double R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1}, b[3] = {0, 0, 0};
@@ -709,7 +744,8 @@ public:
     // the relocalisation table loadMap or the loss built, or builds it for a tracking session.  The table is then neither
     // rebuilt nor re-versioned until the mode ends.  Disabling is always allowed: mapping resumes on the next keyframe
     // decision, ids continue from the counters, and a frame still lost gets max_lost_frames frames from then on.
-    // configure, reset, setPreset, setDistortion and setFisheye end the mode; loadMap keeps it (the loaded map is frozen).
+    // configure, reset, setPreset, setDistortion, setFisheye and setDistortionCoeffs end the mode; loadMap keeps it (the loaded map
+    // is frozen).
     int setLocalisationOnly(bool on) {
         if (!on) {
             if (frozen && lost) lost_frames = 0;
@@ -755,6 +791,14 @@ public:
         n_lens_drops = 0;
         reset();
     }
+    // OpenCV's distortion vector (Camera::setDistortionCoeffs); replaces either model above and is replaced by them.  False, with
+    // nothing changed, for a vector the camera refuses.
+    bool setDistortionCoeffs(const double* c, int n) {
+        if (!cam.setDistortionCoeffs(c, n)) return false;
+        n_lens_drops = 0;
+        reset();
+        return true;
+    }
 
     void reset() {   // System::reset (system.cpp:42-55)
         cur.reset();
@@ -787,7 +831,8 @@ public:
         std::sort(mp_ids.begin(), mp_ids.end());
         w.raw("ALMP", 4); w.u32(MAP_VERSION); w.u64(0); w.u32((uint32_t)kf_ids.size()); w.u32((uint32_t)mp_ids.size());
         w.i32(cam.w); w.i32(cam.h); w.f64(cam.fx); w.f64(cam.fy); w.f64(cam.cx); w.f64(cam.cy); w.i32(cam.lens);
-        for (int i = 0; i < 4; i++) w.f64(cam.dist[i]);
+        if (cam.lens == Camera::FULL) for (int i = 0; i < 14; i++) w.f64(cam.full.k[i]);   // lens 3: the 14 coefficients
+        else for (int i = 0; i < 4; i++) w.f64(cam.dist[i]);
         w.i32(cell);
         w.i32(n_kf_ids); w.i32(n_mp_ids); w.i32(n_kf);
         w.se3(cur.Twc);
@@ -1148,14 +1193,15 @@ private:
         if (!r.u64(total) || total != (uint64_t)bytes) return fail("byte count differs from the blob's length");
         if (!r.u32(nkf) || !r.u32(nmp)) return fail("truncated header");
         int32_t w = 0, h = 0, lens = 0, cs = 0;
-        double K[4], D[4];
+        double K[4], D[14];
         bool ok = r.i32(w) && r.i32(h);
         for (int i = 0; i < 4; i++) ok = ok && r.f64(K[i]);
         ok = ok && r.i32(lens);
-        for (int i = 0; i < 4; i++) ok = ok && r.f64(D[i]);
+        const int nd = lens == Camera::FULL ? 14 : 4;   // lens 3 carries the whole vector
+        for (int i = 0; i < nd; i++) ok = ok && r.f64(D[i]);
         if (!ok) return fail("truncated or non-finite camera section");
         bool same = w == cam.w && h == cam.h && K[0] == cam.fx && K[1] == cam.fy && K[2] == cam.cx && K[3] == cam.cy && lens == cam.lens;
-        for (int i = 0; i < 4; i++) same = same && D[i] == cam.dist[i];
+        for (int i = 0; i < nd; i++) same = same && D[i] == (nd == 14 ? cam.full.k[i] : cam.dist[i]);
         if (!same) return fail("camera or lens differs from the configured one");
         if (!r.i32(cs)) return fail("truncated grid section");
         if (cs != cell) return fail("grid cell size differs from the preset's");
@@ -1481,6 +1527,8 @@ private:
         m.nkp3d = frame.n3d;
         m.has_dist = cam.has_dist;
         m.fisheye = cam.lens == Camera::FISHEYE;
+        m.full = cam.lens == Camera::FULL;
+        if (m.full) m.lf = cam.full;
         for (int i = 0; i < 4; i++) m.dist[i] = cam.dist[i];
         // the frame's keypoints cell by cell, each cell in its insertion order (what Frame::getSurroundingKeypoints walks)
         std::unordered_map<int, int> mp_index;

@@ -74,6 +74,10 @@ _OPTIONAL = {
                                   _vp, _vp, _i32, _vp, _vp, _vp, C.c_float, _vp, _vp],
     "alva_k_undistort_points_fisheye": [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp],
     "alva_k_project_points_fisheye": [_vp, _vp, _i32, _vp, _vp, _vp],
+    "alva_k_undistort_points_full": [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _i32, _vp],
+    "alva_k_project_points_full": [_vp, _vp, _i32, _vp, _vp, _i32, _vp],
+    "alva_k_match_to_map_full": [_vp, _i32, _i32, _i32, C.c_double, C.c_double, C.c_double, C.c_double, _vp, _i32, _vp, _vp, _i32, _i32,
+                                 _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, C.c_float, C.c_float, _vp, _vp, _vp, _vp, _i32],
     "alva_k_rotate_priors": [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _i32, _vp, _vp, _vp],
     "alva_k_p3p_lmeds": [_vp, _i32, _i32, _vp, _vp, _vp, _i32, C.c_float, C.c_float, C.c_float, C.c_uint32, _vp, _vp, _vp],
     "alva_k_p3p_ransac": [_vp, _i32, _i32, _vp, _vp, _vp, _i32, C.c_float, C.c_float, C.c_float, C.c_uint32, _vp, _vp, _vp],
@@ -122,6 +126,20 @@ def _ptr(t):
 def _f64x4(v):
     """four host doubles (intrinsics or distortion coefficients)"""
     return (C.c_double * 4)(*[float(x) for x in v])
+
+
+def _f64n(v):
+    """host doubles of any length (an OpenCV distortion vector)"""
+    v = [float(x) for x in v]
+    return (C.c_double * len(v))(*v)
+
+
+def _f64x14(v):
+    """an OpenCV distortion vector of 4, 5, 8, 12 or 14 entries zero-padded to the 14 host doubles a lens-3 call reads"""
+    v = [float(x) for x in v]
+    if len(v) not in (4, 5, 8, 12, 14):
+        raise ValueError(f"an OpenCV distortion vector has 4, 5, 8, 12 or 14 entries, not {len(v)}")
+    return (C.c_double * 14)(*(v + [0.0] * (14 - len(v))))
 
 
 class Context:
@@ -230,15 +248,21 @@ class Context:
         self._chk(self.L.alva_k_corner_subpix(self.h, _ptr(gray), w, h, nframes, _ptr(pts), _ptr(counts), cap))
 
     def match_to_map(self, w, h, cell, K, Twc_cur, kp_mp, kp_px, nkp3d, kf_Twc, mp_wpt, mp_is3d, obs_start, obs_kf, obs_px,
-                     desc_start, desc, local_mp, kp_match, kp_dist, n_match, max_proj_err=2.0, dist_ratio=0.2, dist=None, fisheye=None):
+                     desc_start, desc, local_mp, kp_match, kp_dist, n_match, max_proj_err=2.0, dist_ratio=0.2, dist=None, fisheye=None,
+                     coeffs=None):
         """Mapper::matchToMap on flat device arrays -- see alva_k_match_to_map; dist = (k1, k2, p1, p2): the lens-distorted
         projections of alva_k_match_to_map_dist; fisheye = (k1, k2, k3, k4): those of the equidistant fisheye model
-        (alva_k_match_to_map_fisheye)."""
+        (alva_k_match_to_map_fisheye); coeffs = OpenCV's 4- to 14-entry vector: alva_k_match_to_map_full."""
         args = (self.h, w, h, cell, K[0], K[1], K[2], K[3], _ptr(Twc_cur), kp_mp.numel(), _ptr(kp_mp), _ptr(kp_px), nkp3d,
                 kf_Twc.shape[0], _ptr(kf_Twc), mp_wpt.shape[0], _ptr(mp_wpt), _ptr(mp_is3d), _ptr(obs_start), _ptr(obs_kf),
                 _ptr(obs_px), _ptr(desc_start), _ptr(desc), local_mp.numel(), _ptr(local_mp), max_proj_err, dist_ratio,
                 _ptr(kp_match), _ptr(kp_dist), _ptr(n_match))
-        if fisheye is not None:
+        if coeffs is not None:
+            if dist is not None or fisheye is not None:
+                raise ValueError("match_to_map: coeffs, dist and fisheye are three lens models; give one")
+            c = _f64n(coeffs)
+            self._chk(self.L.alva_k_match_to_map_full(*args, c, len(c)))
+        elif fisheye is not None:
             if dist is not None:
                 raise ValueError("match_to_map: dist and fisheye are two lens models; give one")
             self._chk(self.L.alva_k_match_to_map_fisheye(*args, _f64x4(fisheye)))
@@ -252,8 +276,9 @@ class Context:
         """the frozen map's re-acquisition of fresh detections -- see alva_k_match_frame_to_map.  Device tensors: Twc [7] float64,
         wpt [n][3] float64, desc_start [n + 1] int32, desc [rows][32] uint8, skip [n] uint8 or None, q_px [nq][2] float32,
         q_desc [nq][32] uint8, q_kept [nq] uint8; out q_row / q_dist [nq] int32.  lens 0 pinhole, 1 radial-tangential, 2 fisheye
-        with coef = its four coefficients."""
-        self._chk(self.L.alva_k_match_frame_to_map(self.h, w, h, cell, K[0], K[1], K[2], K[3], lens, _f64x4(coef) if lens else None,
+        with coef = its four coefficients, 3 OpenCV's whole vector with coef = its 4 to 14 coefficients (zero-padded here)."""
+        cf = (_f64x14(coef) if lens == 3 else _f64x4(coef)) if lens else None
+        self._chk(self.L.alva_k_match_frame_to_map(self.h, w, h, cell, K[0], K[1], K[2], K[3], lens, cf,
                                                    _ptr(Twc), wpt.shape[0], _ptr(wpt), _ptr(desc_start), _ptr(desc), _ptr(skip),
                                                    q_px.shape[0], _ptr(q_px), _ptr(q_desc), _ptr(q_kept), float(radius), _ptr(q_row),
                                                    _ptr(q_dist)))
@@ -277,11 +302,24 @@ class Context:
         """cv::fisheye::projectPoints of the float points (x/z, y/z, 1) -- see alva_k_project_points_fisheye."""
         self._chk(self.L.alva_k_project_points_fisheye(self.h, _ptr(Xc), n, _f64x4(K), _f64x4(k4), _ptr(uv)))
 
+    def undistort_points_full(self, px, counts, nframes, cap, K, coeffs, unpx):
+        """cv::undistortPoints(px, unpx, K, D, K) with OpenCV's whole distortion vector D = coeffs (4, 5, 8, 12 or 14 entries) --
+        see alva_k_undistort_points_full."""
+        c = _f64n(coeffs)
+        self._chk(self.L.alva_k_undistort_points_full(self.h, _ptr(px), _ptr(counts), nframes, cap, _f64x4(K), c, len(c), _ptr(unpx)))
+
+    def project_points_full(self, Xc, n, K, coeffs, uv):
+        """cv::projectPoints of the float points (x/z, y/z, 1) with OpenCV's whole distortion vector -- see
+        alva_k_project_points_full."""
+        c = _f64n(coeffs)
+        self._chk(self.L.alva_k_project_points_full(self.h, _ptr(Xc), n, _f64x4(K), c, len(c), _ptr(uv)))
+
     def rotate_priors(self, bv, flag, n, w, h, K, D4, lens, R9, prior, rotated):
         """System's gyro-rotated KLT priors -- see alva_k_rotate_priors; K / D4 (None: zeros) / R9 on the host, lens 0 pinhole,
-        1 radial-tangential, 2 fisheye."""
+        1 radial-tangential, 2 fisheye, 3 OpenCV's whole vector (D4 then its 4 to 14 coefficients, zero-padded here)."""
         R = (C.c_double * 9)(*[float(v) for v in R9])
-        self._chk(self.L.alva_k_rotate_priors(self.h, _ptr(bv), _ptr(flag), n, w, h, _f64x4(K), None if D4 is None else _f64x4(D4), lens, R,
+        D = None if D4 is None else (_f64x14(D4) if lens == 3 else _f64x4(D4))
+        self._chk(self.L.alva_k_rotate_priors(self.h, _ptr(bv), _ptr(flag), n, w, h, _f64x4(K), D, lens, R,
                                               _ptr(prior), _ptr(rotated)))
 
     def p3p_lmeds(self, nprob, cap, bvs, wpts, counts, Twc_out, outlier, info=None, max_iter=100, err_px=3.0, fx=1.0, fy=1.0,

@@ -5,7 +5,8 @@
             1280x720 view, so 1000 features/frame is always reachable.
 * frames  : a pinhole camera on a smooth seeded SE(3) trajectory (about 3 px/frame lateral motion, +-0.2 deg/frame
             rotation) looking at the texture plane z = 4; bilinear sampling; RGBA with R = G = B, A = 255.  Optionally
-            through OpenCV's radial-tangential lens (k1, k2, p1, p2) or its equidistant fisheye lens (k1, k2, k3, k4).
+            through OpenCV's radial-tangential lens (k1, k2, p1, p2), its whole distortion vector (up to 14 entries) or its
+            equidistant fisheye lens (k1, k2, k3, k4).
 * descriptors / BA problems for the matcher and bundle-adjustment stages.
 Pure numpy (+ scipy.ndimage for the blur); nothing here is on the product path.
 """
@@ -81,6 +82,41 @@ def undistort_normalised(xd, yd, dist, tol=1e-12, max_iter=500):
     raise ValueError(f"lens model {dist} does not invert over this image")
 
 
+def tilt_matrices(tau_x, tau_y):
+    """OpenCV's matTilt and invMatTilt of a tilted sensor (detail::computeTiltProjectionMatrix): the identity for zero angles"""
+    if tau_x == 0 and tau_y == 0:
+        return np.eye(3), np.eye(3)
+    cx, sx, cy, sy = np.cos(tau_x), np.sin(tau_x), np.cos(tau_y), np.sin(tau_y)
+    R = np.array([[cy, 0, -sy], [0, 1, 0], [sy, 0, cy]]) @ np.array([[1, 0, 0], [0, cx, sx], [0, -sx, cx]])
+    tilt = np.array([[R[2, 2], 0, -R[0, 2]], [0, R[2, 2], -R[1, 2]], [0, 0, 1]]) @ R
+    inv = 1.0 / R[2, 2]
+    itilt = R.T @ np.array([[inv, 0, inv * R[0, 2]], [0, inv, inv * R[1, 2]], [0, 0, 1]])
+    return tilt, itilt
+
+
+def undistort_normalised_full(xd, yd, coeffs, tol=1e-12, max_iter=1000):
+    """The normalised point (x, y) that OpenCV's model with its whole distortion vector (4 to 14 entries: k1 k2 p1 p2 k3 k4 k5 k6
+    s1 s2 s3 s4 tau_x tau_y) maps to (xd, yd): the tilt undone with invMatTilt, then cv::undistortPoints' fixed-point step with
+    the rational denominator and the thin-prism terms, run to convergence (scene generation, not the 5-iteration library call)."""
+    k = np.zeros(14)
+    k[:len(coeffs)] = coeffs
+    _, itilt = tilt_matrices(k[12], k[13])
+    t = np.stack([xd, yd, np.ones_like(xd)], -1) @ itilt.T
+    x0, y0 = t[..., 0] / t[..., 2], t[..., 1] / t[..., 2]
+    x, y = x0.copy(), y0.copy()
+    for _ in range(max_iter):
+        r2 = x * x + y * y
+        icdist = (1 + ((k[7] * r2 + k[6]) * r2 + k[5]) * r2) / (1 + ((k[4] * r2 + k[1]) * r2 + k[0]) * r2)
+        dx = 2 * k[2] * x * y + k[3] * (r2 + 2 * x * x) + k[8] * r2 + k[9] * r2 * r2
+        dy = k[2] * (r2 + 2 * y * y) + 2 * k[3] * x * y + k[10] * r2 + k[11] * r2 * r2
+        nx, ny = (x0 - dx) * icdist, (y0 - dy) * icdist
+        done = max(np.abs(nx - x).max(), np.abs(ny - y).max()) < tol
+        x, y = nx, ny
+        if done:
+            return x, y
+    raise ValueError(f"lens model {tuple(coeffs)} does not invert over this image")
+
+
 def fisheye_theta(theta_d, k, tol=1e-14, max_iter=200):
     """The incidence angle theta that OpenCV's equidistant fisheye model (k1, k2, k3, k4) maps to theta_d = theta (1 + k1 theta^2
     + k2 theta^4 + k3 theta^6 + k4 theta^8): Newton's method run to convergence (scene generation, not cv::fisheye's 10 steps)."""
@@ -99,9 +135,10 @@ def fisheye_theta(theta_d, k, tol=1e-14, max_iter=200):
     raise ValueError(f"fisheye model {k} does not invert over this image below 90 degrees")
 
 
-def render_gray(tex, pose, w, h, plane_z=4.0, tex_scale=None, dist=None, fisheye=None):
+def render_gray(tex, pose, w, h, plane_z=4.0, tex_scale=None, dist=None, fisheye=None, dist_full=None):
     """Bilinear render of the texture plane z = plane_z seen from pose (R_wc, t_wc); dist = (k1, k2, p1, p2): through that lens;
-    fisheye = (k1, k2, k3, k4): through OpenCV's equidistant fisheye lens instead."""
+    fisheye = (k1, k2, k3, k4): through OpenCV's equidistant fisheye lens instead; dist_full: through OpenCV's whole distortion
+    vector (4 to 14 entries)."""
     fx, fy, cx, cy = intrinsics(w, h)
     if tex_scale is None:
         tex_scale = fx / plane_z          # texture pixels per world unit: ~1 texel per image pixel
@@ -113,6 +150,9 @@ def render_gray(tex, pose, w, h, plane_z=4.0, tex_scale=None, dist=None, fisheye
         theta = fisheye_theta(theta_d, fisheye)
         scale = np.where(theta_d > 0, np.tan(theta) / np.where(theta_d > 0, theta_d, 1.0), 1.0)
         rays = np.stack([xd * scale, yd * scale, np.ones_like(u)], -1) @ R.T
+    elif dist_full is not None:
+        x, y = undistort_normalised_full((u - cx) / fx, (v - cy) / fy, dist_full)
+        rays = np.stack([x, y, np.ones_like(u)], -1) @ R.T
     elif dist is None:
         rays = np.stack([(u - cx) / fx, (v - cy) / fy, np.ones_like(u)], -1) @ R.T
     else:
@@ -144,15 +184,16 @@ def gray_to_rgba(g):
     return out
 
 
-def make_frames(nframes, w, h, seed=99, rgba=True, texture_seed=1234, dist=None, fisheye=None):
+def make_frames(nframes, w, h, seed=99, rgba=True, texture_seed=1234, dist=None, fisheye=None, dist_full=None):
     """`seed` picks the camera path, `texture_seed` the scene (two calls with the same texture_seed look at the same plane);
     dist = (k1, k2, p1, p2) renders through OpenCV's radial-tangential lens with the intrinsics() camera (None: a pinhole);
-    fisheye = (k1, k2, k3, k4) through OpenCV's equidistant fisheye lens with the same camera matrix."""
-    if dist is not None and fisheye is not None:
-        raise ValueError("make_frames: dist and fisheye are two lens models; give one")
+    fisheye = (k1, k2, k3, k4) through OpenCV's equidistant fisheye lens with the same camera matrix; dist_full = OpenCV's whole
+    distortion vector (4 to 14 entries) through that model."""
+    if sum(v is not None for v in (dist, fisheye, dist_full)) > 1:
+        raise ValueError("make_frames: dist, fisheye and dist_full are three lens models; give one")
     tex = make_texture(seed=texture_seed)
     poses = trajectory(nframes, w, h, seed)
-    frames = [render_gray(tex, p, w, h, dist=dist, fisheye=fisheye) for p in poses]
+    frames = [render_gray(tex, p, w, h, dist=dist, fisheye=fisheye, dist_full=dist_full) for p in poses]
     g = np.stack(frames)
     return (gray_to_rgba(g) if rgba else g), poses
 

@@ -20,6 +20,7 @@ def _bind():
     L.alva_system_set_clahe.argtypes = [_vp, _i32, _f64, _i32]
     L.alva_system_set_distortion.argtypes = [_vp] + [_f64] * 4
     L.alva_system_set_fisheye.argtypes = [_vp, _i32] + [_f64] * 4
+    L.alva_system_set_distortion_coeffs.argtypes = [_vp, _vp, _i32]
     L.alva_system_lens_drops.argtypes = [_vp]
     L.alva_system_set_preset.argtypes = [_vp, _i32]
     L.alva_system_set_relocalisation.argtypes = [_vp, _i32]
@@ -176,6 +177,17 @@ class System:
         rc = self.L.alva_system_set_fisheye(self.h, 1 if enabled else 0, float(k1), float(k2), float(k3), float(k4))
         if rc != 0:
             raise AlvaError(f"alva_system_set_fisheye -> {rc}: {self.L.alva_last_error().decode()}")
+
+    def set_distortion_coeffs(self, coeffs):
+        """OpenCV's whole distortion vector, as cv::calibrateCamera returns it: 4, 5, 8, 12 or 14 entries of (k1, k2, p1, p2, k3,
+        k4, k5, k6, s1, s2, s3, s4, tau_x, tau_y) -- k3, the rational, thin-prism and tilted models.  All zero is the pinhole; only
+        k1..p2 non-zero is exactly set_distortion(k1, k2, p1, p2).  Replaces set_distortion's and set_fisheye's models (and is
+        replaced by them); resets the tracker and the map; survives reset() and set_preset(); configuring clears it.  AlvaError
+        (nothing changed) for another length, a non-finite value or |tau_x| or |tau_y| >= pi/2."""
+        c = np.ascontiguousarray(np.asarray(coeffs, np.float64).ravel())
+        rc = self.L.alva_system_set_distortion_coeffs(self.h, c.ctypes.data_as(_vp), len(c))
+        if rc != 0:
+            raise AlvaError(f"alva_system_set_distortion_coeffs -> {rc}: {self.L.alva_last_error().decode()}")
 
     def lens_drops(self):
         """keypoints dropped because the fisheye model could not undistort them, since configuring or the last lens change"""

@@ -108,10 +108,21 @@ int alva_k_project_points(alva_ctx*, const double* Xc, int n, const double* K4, 
 int alva_k_undistort_points_fisheye(alva_ctx*, const float* px, const int32_t* counts, int nframes, int cap, const double* K4,
                                     const double* D4, float* unpx);
 int alva_k_project_points_fisheye(alva_ctx*, const double* Xc, int n, const double* K4, const double* D4, float* uv);
+/* The same two calls with OpenCV's whole distortion vector: coeffs (HOST) holds ncoeffs = 4, 5, 8, 12 or 14 entries of
+ * {k1, k2, p1, p2, k3, k4, k5, k6, s1, s2, s3, s4, tau_x, tau_y} (what cv::calibrateCamera returns by default and with
+ * CALIB_RATIONAL_MODEL, CALIB_THIN_PRISM_MODEL or CALIB_TILTED_MODEL), zero-padded to 14.  The tilt matrices of a non-zero
+ * tau_x / tau_y are built once on the host, as OpenCV builds them.  Same shapes, layout, counts and checks as
+ * alva_k_undistort_points / alva_k_project_points, and bit-exact with cv::undistortPoints / cv::projectPoints of the vector;
+ * (k1, k2, p1, p2) padded with zeros gives exactly their bits.  ALVA_E_INVALID also for another ncoeffs, a non-finite
+ * coefficient, or |tau_x| or |tau_y| >= pi/2. */
+int alva_k_undistort_points_full(alva_ctx*, const float* px, const int32_t* counts, int nframes, int cap, const double* K4,
+                                 const double* coeffs, int ncoeffs, float* unpx);
+int alva_k_project_points_full(alva_ctx*, const double* Xc, int n, const double* K4, const double* coeffs, int ncoeffs, float* uv);
 /* The rotation-compensated KLT priors of System's gyro mode (alva_system_set_gyro; not in the reference).  For every point i with
  * flag[i] != 0: c = R^T bv[i] (bv [n][3] double, the keypoint's bearing in the previous camera; R9 row-major, the camera's
  * rotation from the previous frame to the current one, HOST array), projected through the lens -- 0 the pinhole, 1 the
- * radial-tangential model (alva_k_project_points), 2 the fisheye model (alva_k_project_points_fisheye) -- and written to
+ * radial-tangential model (alva_k_project_points), 2 the fisheye model (alva_k_project_points_fisheye), 3 the full vector
+ * (alva_k_project_points_full; D4 then holds all 14 coefficients) -- and written to
  * prior [n][2] float (8-byte aligned) with rotated[i] = 1 only when c.z > 0 and the projection lies inside the w x h image
  * (0 <= u < w, 0 <= v < h).  Every other point keeps its prior, with rotated[i] = 0.  K4 / D4 / R9 are host arrays (D4 NULL:
  * zeros); bv, flag, prior, rotated are device arrays; n = 0 is a no-op.  Bit-exact with the host build of the same arithmetic
@@ -332,10 +343,19 @@ int alva_k_match_to_map_fisheye(alva_ctx*, int w, int h, int cell, double fx, do
                                 const float* obs_px, const int32_t* desc_start, const uint8_t* desc, int n_local, const int32_t* local_mp,
                                 float max_proj_err, float dist_ratio, int32_t* kp_match, float* kp_dist, int32_t* n_match,
                                 const double* fisheye4);
+/* The same through OpenCV's whole distortion vector (coeffs / ncoeffs as alva_k_undistort_points_full, HOST): the map point and
+ * the co-projection errors are projected as alva_k_project_points_full does.  ALVA_E_INVALID for a vector it refuses. */
+int alva_k_match_to_map_full(alva_ctx*, int w, int h, int cell, double fx, double fy, double cx, double cy, const double* Twc_cur,
+                             int n_kp, const int32_t* kp_mp, const float* kp_px, int nkp3d, int n_kf, const double* kf_Twc, int n_mp,
+                             const double* mp_wpt, const uint8_t* mp_is3d, const int32_t* obs_start, const int32_t* obs_kf,
+                             const float* obs_px, const int32_t* desc_start, const uint8_t* desc, int n_local, const int32_t* local_mp,
+                             float max_proj_err, float dist_ratio, int32_t* kp_match, float* kp_dist, int32_t* n_match,
+                             const double* coeffs, int ncoeffs);
 /* Projection-gated matching of a tracked frame's fresh detections against a frozen map table (the re-acquisition of
  * alva_system_set_localisation_only; not in the reference).  The gates of Mapper::matchToMap (mapper.cpp:354-587) for queries
- * without a map point of their own.  Device pointers except coef4 (HOST, required for lens 1 / 2):
- *   camera w, h, fx, fy, cx, cy; lens 0 pinhole, 1 radial-tangential (k1 k2 p1 p2), 2 fisheye (k1..k4); cell: the grid cell
+ * without a map point of their own.  Device pointers except coef4 (HOST, required for lens 1 / 2 / 3):
+ *   camera w, h, fx, fy, cx, cy; lens 0 pinhole, 1 radial-tangential (k1 k2 p1 p2), 2 fisheye (k1..k4), 3 OpenCV's whole
+ *   vector (coef4 then holds 14 coefficients, as alva_k_undistort_points_full's); cell: the grid cell
  *   Twc [7] = [t, q(x,y,z,w)] of the frame
  *   table (the relocalisation table's layout, ascending map point id): wpt [n_mp][3] FP64, CSR desc_start [n_mp + 1] ->
  *   desc [rows][32] (16-byte aligned); skip [n_mp] (optional): 1 = leave the row out (map points the frame already tracks)
@@ -530,8 +550,19 @@ int  alva_system_set_distortion(alva_system*, double k1, double k2, double p1, d
  * before configure; ALVA_E_INVALID for a null handle or a non-finite coefficient.  Fields of view of 180 degrees or more are
  * out of its range (OpenCV clamps theta_d to pi/2). */
 int  alva_system_set_fisheye(alva_system*, int enabled, double k1, double k2, double k3, double k4);
+/* OpenCV's whole distortion vector for a configured System: coeffs (HOST) holds n = 4, 5, 8, 12 or 14 entries of
+ * {k1, k2, p1, p2, k3, k4, k5, k6, s1, s2, s3, s4, tau_x, tau_y}, as cv::calibrateCamera returns them (5 by default; 8, 12, 14
+ * with CALIB_RATIONAL_MODEL, CALIB_THIN_PRISM_MODEL, CALIB_TILTED_MODEL).  All zero selects the pinhole; only k1 k2 p1 p2
+ * non-zero is exactly set_distortion(k1, k2, p1, p2), in every bit of the trace and the map blob; anything else applies
+ * cv::undistortPoints / cv::projectPoints with the whole vector wherever set_distortion's model is applied, bit-exact on the
+ * device (alva_k_undistort_points_full).  Like the radial-tangential model it never fails (where it folds back, the pinhole
+ * point), so alva_system_lens_drops stays 0.  set_distortion, set_fisheye and set_distortion_coeffs each replace the others'
+ * model; it resets the tracker and the map (ending localisation-only); configure clears it; reset, set_preset, set_clahe,
+ * set_relocalisation and set_gyro keep it.  ALVA_E_STATE before configure; ALVA_E_INVALID for a null handle, another n, a
+ * non-finite coefficient or |tau_x| or |tau_y| >= pi/2.  A refusal changes nothing. */
+int  alva_system_set_distortion_coeffs(alva_system*, const double* coeffs, int n);
 /* keypoints dropped because the fisheye model could not undistort them, since configure or the last set_distortion /
- * set_fisheye (always 0 for the pinhole and radial-tangential lenses) */
+ * set_fisheye / set_distortion_coeffs (always 0 for the pinhole, the radial-tangential lens and OpenCV's whole vector, lens 3) */
 int  alva_system_lens_drops(alva_system*);
 /* The reference's three tuned configurations (state.hpp:9-17), and DEFAULT = what configure sets (system.cpp:15-19):
  *              grid cell  CLAHE (clip 3, tile 50)  keyframe filtering ratio  P3P on every tracked frame
@@ -630,7 +661,8 @@ int  alva_system_gyro_stats(alva_system*, int32_t* out5, double* dR9);
  *
  * Format, version 1: little-endian, fixed-width fields, no padding (i32 / u32 / u64 / f32 / f64, u8 flags 0 or 1).
  *   header     "ALMP", u32 version = 1, u64 total bytes, u32 keyframe count, u32 map point count
- *   camera     i32 w, h; f64 fx, fy, cx, cy; i32 lens (0 pinhole, 1 radial-tangential, 2 fisheye); f64 coefficients [4]
+ *   camera     i32 w, h; f64 fx, fy, cx, cy; i32 lens (0 pinhole, 1 radial-tangential, 2 fisheye, 3 OpenCV's whole vector);
+ *              f64 coefficients [4] for lenses 0..2, [14] for lens 3
  *   grid       i32 cell size of the preset
  *   counters   i32 n_kf_ids, n_mp_ids (the next ids), n_kf (= the keyframe count)
  *   pose       f64 t [3], q [4] (x y z w): the pose the lost frames report

@@ -38,6 +38,7 @@ public:
     // not in the reference's class: OpenCV's equidistant fisheye lens (k1..k4 on theta; enabled = 0: the pinhole), for
     // wide-angle cameras; resets the tracker and the map; 0 or an ALVA_E_* code
     int setFisheye(int enabled, double k1, double k2, double k3, double k4) { return alva_system_set_fisheye(h_, enabled, k1, k2, k3, k4); }
+    int setDistortionCoeffs(const double* coeffs, int n) { return alva_system_set_distortion_coeffs(h_, coeffs, n); }
     // not in the reference's class: the map as bytes (alva_system_save_map / alva_system_load_map, alva_b200.h).  saveMap
     // replaces `out` with the blob; loadMap needs setRelocalisation > 0 and enters the lost state.  0 or an ALVA_E_* code
     // (one serialisation when `out`'s capacity already holds the map, e.g. when it is reused from call to call)
