@@ -202,7 +202,10 @@ template <> struct Acc<0> {
     static __device__ __forceinline__ int to_int(int v) { return v; }
     // (256 - dot) << 21 | idx as one multiply-add: dot * -(2^21) + ((256 << 21) + idx)  (idx < 2^22, (256 - dot) even)
     static __device__ __forceinline__ uint32_t key(int v, int idx) { return (uint32_t)v * 0xFFE00000u + ((256u << 21) + (uint32_t)idx); }
-    static __device__ __forceinline__ int dot_of_key(uint32_t k) { return 256 - (int)(k >> 21); }   // NONE -> -1791: below every dot product
+    // NONE -> -1791: below every dot product.  Bit 21 of the key is bit 21 of the index, so for an index >= 2^21 this is the dot
+    // product minus one.  That only lowers the bound thr built from it: the filter then lets through candidates it could have
+    // skipped (at most ones of the bound's own distance, which lose to it by index in the insertion), never drops one that matters.
+    static __device__ __forceinline__ int dot_of_key(uint32_t k) { return 256 - (int)(k >> 21); }
     static __device__ __forceinline__ void mma(int (&d)[64], uint64_t da, uint64_t db, uint32_t acc) { wgmma_i8(d, da, db, acc); }
 };
 template <> struct Acc<1> {
@@ -211,7 +214,7 @@ template <> struct Acc<1> {
     // the accumulators are integer-valued floats of magnitude <= 256: adding 1.5 * 2^23 leaves the integer in the low mantissa bits
     static __device__ __forceinline__ int to_int(float v) { return __float_as_int(v + 12582912.0f) - 0x4B400000; }
     static __device__ __forceinline__ uint32_t key(float v, int idx) { return (uint32_t)to_int(v) * 0xFFE00000u + ((256u << 21) + (uint32_t)idx); }
-    static __device__ __forceinline__ float dot_of_key(uint32_t k) { return (float)(256 - (int)(k >> 21)); }
+    static __device__ __forceinline__ float dot_of_key(uint32_t k) { return (float)(256 - (int)(k >> 21)); }   // as Acc<0>
     static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) { wgmma_e4m3(d, da, db, acc); }
 };
 

@@ -181,11 +181,14 @@ int alva_k_orb_detect(alva_ctx*, const uint8_t* gray, int w, int h, int nframes,
 
 /* Brute-force Hamming 2-NN (BFMatcher(NORM_HAMMING).knnMatch(k=2), features2d/src/matchers.cpp:757;
  * tie rule core/src/batch_distance.cpp:235-248).  q: [nq][32], t: [nt][32] bytes;
- * out[4*i] = {idx0, dist0, idx1, dist1} (int32; -1 when nt < 2). */
+ * out[4*i] = {idx0, dist0, idx1, dist1} (int32; -1 when nt < 2).  DEVICE pointers, each 16-byte aligned; nq >= 1 and
+ * 1 <= nt < 2^22 (a key holds a 22-bit train index), else ALVA_E_INVALID before anything runs. */
 int alva_k_hamming_knn2(alva_ctx*, const uint8_t* q, int nq, const uint8_t* t, int nt, int32_t* out);
 
-/* Batched variant: q is [nbatch][qcap][32] of which only the first counts[b] slots of batch b are live (qcap a
- * multiple of 8); dead slots come back as -1. */
+/* Batched variant: q is [nbatch][qcap][32] of which only the first counts[b] slots of batch b are live (nbatch >= 1, qcap a
+ * positive multiple of 8); out is [nbatch][qcap][4].  counts (device memory) are clamped to [0, qcap]: a count above qcap makes
+ * every slot of its batch live, a negative one none.  Every dead slot comes back as four -1s.  Pointers and the limits on nt as
+ * alva_k_hamming_knn2. */
 int alva_k_hamming_knn2_batch(alva_ctx*, const uint8_t* q, const int32_t* counts, int nbatch, int qcap,
                               const uint8_t* t, int nt, int32_t* out);
 
@@ -432,7 +435,8 @@ int alva_k_ba_local(alva_ctx*, int nprob, int nkf, int nlm, int nobs, const doub
  * int8, wgmma s8 x s8 -> s32, dot = 256 - 2 * distance): 0 never, 1 for large query sets (default), 2 always.  Results
  * are identical.  "knn_mma_kind" = 0 | 1: operand kind of that kernel (0: +-1 as int8, int32 accumulators -- default;
  * 1: +-1.0 as E4M3, fp32 accumulators).  "knn_mma_mode" = 0 | 1 | 2: its
- * shared-memory operand layout (0 no swizzle, 1 128-byte swizzle, 2 debugging variant).
+ * shared-memory operand layout (0 no swizzle, 1 128-byte swizzle, 2 a debugging variant of 0 for the wgmma descriptor
+ * convention, whose results are not guaranteed).
  * "frontend_variant" = 2 | 0: the fused front-end kernel (2: frontend_tile_kernel_v2, default; 0: the round-1 kernel, which
  * also serves geometries a TMA tensor map cannot express).  Results are identical.
  * "frontend_prefetch" = 0 | 1: variant 2 also pulls the tile at the same position a few frames ahead into L2 (TMA prefetch)
