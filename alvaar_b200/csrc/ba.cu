@@ -1777,7 +1777,7 @@ extern "C" int alva_set_option(const char* name, int value) {
     if (name && !strcmp(name, "pipeline_ba_overlap")) return set_option(alva_g_ba_overlap, value ? 1 : 0);
     if (name && !strcmp(name, "knn_qpw") && (value == 4 || value == 8)) return set_option(alva_g_knn_qpw, value);
     if (name && !strcmp(name, "knn_mma") && value >= 0 && value <= 2) return set_option(alva_g_knn_mma, value);
-    if (name && !strcmp(name, "knn_mma_kind") && (value == 0 || value == 1)) return set_option(alva_g_knn_mma_kind, value);
+    if (name && !strcmp(name, "knn_mma_kind") && value >= 0 && value <= 2) return set_option(alva_g_knn_mma_kind, value);
     if (name && !strcmp(name, "knn_mma_mode") && value >= 0 && value <= 2) return set_option(alva_g_knn_mma_mode, value);
     alva_set_error("alva_set_option: unknown option");
     return ALVA_E_INVALID;

@@ -7,23 +7,27 @@
 // Why tensor cores: brute-force Hamming IS a contraction.  With every descriptor bit b expanded to the 8-bit value
 // 2b - 1 (+1 / -1), the dot product of two 256-element rows is  256 - 2 * hamming,  exactly (an int32, or a float whose
 // partial sums are all integers of magnitude <= 256).  So the N_q x N_t distance matrix is one 8-bit GEMM with K = 256, and the
-// integer pipes (which bound the LOP3/POPC kernel of hamming.cu) are left with nothing but the top-2 selection.  Two operand
-// kinds are built: int8 (+-1 as s8, s32 accumulators; the default) and E4M3 (+-1.0, f32 accumulators); the results are
-// bit-identical (every value involved is an exactly representable integer).
+// integer pipes (which bound the LOP3/POPC kernel of hamming.cu) are left with nothing but the top-2 selection.  Hopper's 1-bit
+// MMA (wgmma .b1.and.popc: the sum over K of popc(a AND b)) does the same on a quarter of the operand bytes: with each query row
+// stored as [a | ~a] and each train row as [~b | b] (512 bits), the accumulator is popc(a & ~b) + popc(~a & b), the Hamming
+// distance itself, in 2 wgmma m64n128k256 per tile instead of 8 m64n128k32.  Three operand kinds are built: 1-bit (s32
+// accumulators, distances; the default), int8 (+-1 as s8, s32 accumulators, dot products) and E4M3 (+-1.0, f32 accumulators);
+// the results are bit-identical (every value involved is an exactly representable integer).
 //
 // Shape of the kernel (one CTA per 256 query rows, 1 CTA / SM, 17 warps):
-//   warps 0-15  consumers: 4 warpgroups, one per 64 query rows.  Per train tile each warpgroup issues 8
-//                       wgmma.mma_async m64n128k32 (K = 256) with both operands read from shared memory, waits for them,
+//   warps 0-15  consumers: 4 warpgroups, one per 64 query rows.  Per train tile each warpgroup issues 2 wgmma.mma_async
+//                       m64n128k256 .b1 (8 m64n128k32 for int8 / E4M3) with both operands read from shared memory, waits for them,
 //                       hands the ring stage back, and runs the top-2 selection on the accumulators in its own registers
 //                       while the other warpgroups' MMAs keep the tensor cores busy.  In the accumulator fragment a thread
-//                       holds 32 columns of two rows; it reduces every 8 dot products of a row to their maximum and compares
-//                       the largest of the four with a bound on the row's second best, which the four threads of the row
-//                       share by shuffles once per tile; only the groups above it run the top-2 insertion, on packed keys
-//                       hamming << 22 | index (one multiply-add builds a key, three min / max insert it: OpenCV's strict
+//                       holds 32 columns of two rows; it reduces every 8 values of a row to the nearest (smallest distance,
+//                       or largest dot product) and compares the nearest of the four with a bound on the row's second best,
+//                       which the four threads of the row share by shuffles once per tile; only the groups that beat it run
+//                       the top-2 insertion, on packed keys hamming << 22 | index (one shift-or or multiply-add builds a key,
+//                       three min / max insert it: OpenCV's strict
 //                       '<' with ties to the lowest train index is the unsigned order of those keys).  The selection, not
 //                       the MMAs, bounds the kernel (DESIGN §4.4), so its cost per tile is what these filters cut.  The four
 //                       threads that share a row merge their pairs by shuffles at the end.
-//   warp 16     producer: bulk async copies (cp.async.bulk, the TMA engine's 1-D mode) of pre-tiled 32 KB operand blobs into
+//   warp 16     producer: bulk async copies (cp.async.bulk, the TMA engine's 1-D mode) of pre-tiled 8 KB (1-bit) or 32 KB operand blobs into
 //                       a 4-stage shared-memory ring, completion on mbarriers.
 // The operands are expanded from the packed 256-bit descriptors by knn2_expand_kernel straight into the shared-memory
 // image of a tile (canonical K-major layout), so the producer needs no tensor map and no swizzle pattern has to be
@@ -36,9 +40,12 @@ namespace {
 constexpr int TM = 128;                 // query rows per A tile (two wgmma M = 64 blocks)
 constexpr int TN = 128;                 // train rows per B tile (wgmma N)
 constexpr int WM = 64;                  // query rows per consumer warpgroup (wgmma M)
-constexpr int KBYTES = 256;             // int8 elements per expanded descriptor
-constexpr int BLOB = TM * KBYTES;       // one operand tile in shared memory: 32 KB
-constexpr int NSTAGE = 4;               // train-tile ring
+// bytes per expanded descriptor row, per operand kind: 256 one-byte elements (kinds 0 and 1), or the 512 bits [a | ~a] of a query
+// and [~b | b] of a train row (kind 2)
+__host__ __device__ constexpr int row_bytes(int kind) { return kind == 2 ? 64 : 256; }
+// one operand tile in shared memory: 32 KB (kinds 0 and 1), 8 KB (kind 2)
+__host__ __device__ constexpr int blob_bytes(int kind) { return TM * row_bytes(kind); }
+constexpr int NSTAGE = 4;               // train-tile ring (8 stages measured no faster for kind 2)
 constexpr int CONS_WARPS = 16;          // 4 warpgroups x 64 query rows = 256 rows per CTA
 constexpr int PROD_WARP = CONS_WARPS;
 constexpr int NTHREADS = (CONS_WARPS + 1) * 32;   // + the producer warp
@@ -114,6 +121,27 @@ __device__ __forceinline__ void wgmma_e4m3(float (&d)[64], uint64_t da, uint64_t
           "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
         : "l"(da), "l"(db), "r"(accumulate));
 }
+// D[64 x 128] (+)= popc(A[64 x 256 bits] AND B[128 x 256 bits]) per row pair, both K-major in shared memory (SASS BGMMA)
+__device__ __forceinline__ void wgmma_b1(int (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k256.s32.b1.b1.and.popc "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, "
+        "%46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p;\n"
+        "}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]),
+          "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]),
+          "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]),
+          "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]),
+          "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]),
+          "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]),
+          "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]),
+          "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate));
+}
 
 // ---------------------------------------------------------------------------------------------- operand expansion
 // offsets[b] = number of live queries in batches < b  (counts clamped to [0, qcap]); one small CTA
@@ -152,14 +180,16 @@ __device__ __forceinline__ uint4 expand16(uint32_t v, int kind) {
 
 // One thread per (tile row, 16-byte K chunk).  blockIdx.x < a_blocks: query side (compacting live slots through
 // `offsets`), else train side.  Rows past the end of either side are written as zeros (their dot products are masked
-// / never stored).  rowmap[compact row] = query slot, or -1.
+// / never stored; under kind 2 a zero train row is at distance 0 from every query, so the mask is what keeps it out).
+// rowmap[compact row] = query slot, or -1.
 __global__ void __launch_bounds__(256) knn2_expand_kernel(const uint8_t* __restrict__ q, const int32_t* __restrict__ offsets,
                                                           int nbatch, int qcap, int nq_slots, uint8_t* __restrict__ Aexp,
                                                           int32_t* __restrict__ rowmap, int a_blocks, const uint8_t* __restrict__ t,
                                                           int nt, uint8_t* __restrict__ Bexp, int mode, int kind) {
     const bool is_a = (int)blockIdx.x < a_blocks;
     const int idx = (is_a ? blockIdx.x : blockIdx.x - a_blocks) * 256 + threadIdx.x;
-    const int tile = idx >> 11, wi = idx & 2047, c = wi >> 7, r = wi & 127;
+    const int lg = kind == 2 ? 9 : 11;                        // log2 of the threads per tile: 128 rows x 4 or 16 chunks
+    const int tile = idx >> lg, wi = idx & ((1 << lg) - 1), c = wi >> 7, r = wi & 127;
     const int R = tile * TM + r;
     const uint8_t* src = nullptr;
     if (is_a) {
@@ -179,8 +209,15 @@ __global__ void __launch_bounds__(256) knn2_expand_kernel(const uint8_t* __restr
         if (R < nt) src = t + (size_t)R * 32;
     }
     uint4 o = make_uint4(0u, 0u, 0u, 0u);
-    if (src) o = expand16(*reinterpret_cast<const uint16_t*>(src + 2 * c), kind);
-    uint8_t* dst = (is_a ? Aexp : Bexp) + (size_t)tile * BLOB + tile_offset(mode, r, c);
+    if (src && kind == 2) {
+        // chunks 0, 1: the first 256 bits, a (query) or ~b (train); chunks 2, 3: ~a or b.  popc over [a | ~a] AND [~b | b]
+        // is popc(a & ~b) + popc(~a & b), the Hamming distance
+        o = *reinterpret_cast<const uint4*>(src + 16 * (c & 1));
+        if ((c >> 1) == (is_a ? 1 : 0)) o = make_uint4(~o.x, ~o.y, ~o.z, ~o.w);
+    } else if (src) {
+        o = expand16(*reinterpret_cast<const uint16_t*>(src + 2 * c), kind);
+    }
+    uint8_t* dst = (is_a ? Aexp : Bexp) + (size_t)tile * blob_bytes(kind) + tile_offset(mode, r, c);
     *reinterpret_cast<uint4*>(dst) = o;
 }
 
@@ -194,28 +231,48 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, const MmaLayout& L
     return (uint64_t)lo | ((uint64_t)L.desc_hi << 32);
 }
 
-// accumulator value type per operand kind, and the value <-> key conversions of the epilogue
+// Per operand kind: the accumulator value type, the order of the values (dot products: larger is nearer; distances: smaller
+// is nearer), the value <-> key conversions of the epilogue, and the MMAs of one tile (KSTEPS wgmma, one per 16-byte-chunk pair).
 template <int KIND> struct Acc;
 template <> struct Acc<0> {
     using T = int;
-    static __device__ __forceinline__ int neg() { return NEG; }
+    static constexpr int KSTEPS = 8;
+    static __device__ __forceinline__ int worst() { return NEG; }
+    static __device__ __forceinline__ int best(int a, int b) { return max(a, b); }
+    static __device__ __forceinline__ bool beats(int a, int b) { return a > b; }
     static __device__ __forceinline__ int to_int(int v) { return v; }
     // (256 - dot) << 21 | idx as one multiply-add: dot * -(2^21) + ((256 << 21) + idx)  (idx < 2^22, (256 - dot) even)
     static __device__ __forceinline__ uint32_t key(int v, int idx) { return (uint32_t)v * 0xFFE00000u + ((256u << 21) + (uint32_t)idx); }
     // NONE -> -1791: below every dot product.  Bit 21 of the key is bit 21 of the index, so for an index >= 2^21 this is the dot
     // product minus one.  That only lowers the bound thr built from it: the filter then lets through candidates it could have
     // skipped (at most ones of the bound's own distance, which lose to it by index in the insertion), never drops one that matters.
-    static __device__ __forceinline__ int dot_of_key(uint32_t k) { return 256 - (int)(k >> 21); }
+    static __device__ __forceinline__ int bound_of_key(uint32_t k) { return 256 - (int)(k >> 21); }
     static __device__ __forceinline__ void mma(int (&d)[64], uint64_t da, uint64_t db, uint32_t acc) { wgmma_i8(d, da, db, acc); }
 };
 template <> struct Acc<1> {
     using T = float;
-    static __device__ __forceinline__ float neg() { return (float)NEG; }
+    static constexpr int KSTEPS = 8;
+    static __device__ __forceinline__ float worst() { return (float)NEG; }
+    static __device__ __forceinline__ float best(float a, float b) { return fmaxf(a, b); }
+    static __device__ __forceinline__ bool beats(float a, float b) { return a > b; }
     // the accumulators are integer-valued floats of magnitude <= 256: adding 1.5 * 2^23 leaves the integer in the low mantissa bits
     static __device__ __forceinline__ int to_int(float v) { return __float_as_int(v + 12582912.0f) - 0x4B400000; }
     static __device__ __forceinline__ uint32_t key(float v, int idx) { return (uint32_t)to_int(v) * 0xFFE00000u + ((256u << 21) + (uint32_t)idx); }
-    static __device__ __forceinline__ float dot_of_key(uint32_t k) { return (float)(256 - (int)(k >> 21)); }   // as Acc<0>
+    static __device__ __forceinline__ float bound_of_key(uint32_t k) { return (float)(256 - (int)(k >> 21)); }   // as Acc<0>
     static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) { wgmma_e4m3(d, da, db, acc); }
+};
+// 1-bit operands: the accumulator is the Hamming distance itself (0 .. 256), the key one shift-or
+template <> struct Acc<2> {
+    using T = int;
+    static constexpr int KSTEPS = 2;
+    static __device__ __forceinline__ int worst() { return -NEG; }
+    static __device__ __forceinline__ int best(int a, int b) { return min(a, b); }
+    static __device__ __forceinline__ bool beats(int a, int b) { return a < b; }
+    static __device__ __forceinline__ int to_int(int v) { return v; }
+    static __device__ __forceinline__ uint32_t key(int v, int idx) { return (uint32_t)v << 22 | (uint32_t)idx; }
+    // exact for every index < 2^22; NONE -> 1023, above every distance
+    static __device__ __forceinline__ int bound_of_key(uint32_t k) { return (int)(k >> 22); }
+    static __device__ __forceinline__ void mma(int (&d)[64], uint64_t da, uint64_t db, uint32_t acc) { wgmma_b1(d, da, db, acc); }
 };
 
 // the pair (k0, k1) of two smallest keys absorbs the pair (o0, o1)
@@ -228,10 +285,10 @@ __device__ __forceinline__ void merge2(uint32_t& k0, uint32_t& k1, uint32_t o0, 
 // Top-2 selection over the accumulators of one 64 x 128 tile, n0 = train row of the thread's first column.  Per thread and
 // row: the two smallest keys seen, key = hamming << 22 | index = (256 - dot) << 21 | index -- the lexicographic (distance,
 // index) order of OpenCV's insertion as ONE unsigned compare, so the insertion itself is three min / max and needs no order
-// of arrival.  thr = a dot product the row's final second best is known to reach: a candidate can only matter if its dot
-// product is strictly above it (its index is larger than everything that set the bound).  The row's 32 dot products of the
-// thread are compared as a whole first, then in groups of 8, and only groups above thr run the insertion.  TAIL: the last
-// train tile, whose columns past nt must not be inserted.
+// of arrival.  thr = a value (dot product, or distance under kind 2) the row's final second best is known to reach: a
+// candidate can only matter if it strictly beats it (its index is larger than everything that set the bound).  The row's 32
+// values of the thread are compared as a whole first, then in groups of 8, and only groups that beat thr run the insertion.
+// TAIL: the last train tile, whose columns past nt must not be inserted.
 // fragment: d[4c + 2h + e] = D[r0 + 8h][8c + 2 quad + e], c < 16
 template <class A, bool TAIL>
 __device__ __forceinline__ void top2_rows(const typename A::T (&d)[64], int n0, int nt, uint32_t (&k0)[2], uint32_t (&k1)[2],
@@ -241,21 +298,21 @@ __device__ __forceinline__ void top2_rows(const typename A::T (&d)[64], int n0, 
     for (int h = 0; h < 2; h++) {
         // The four threads of a row share their bounds: a thread's second best is a candidate of the row, so the row's final
         // second best is at least as good, and every column of this tile has a larger index than the earlier tiles' columns.
-        thr[h] = max(thr[h], __shfl_xor_sync(0xffffffffu, thr[h], 1));
-        thr[h] = max(thr[h], __shfl_xor_sync(0xffffffffu, thr[h], 2));
-        T gmax[4];
+        thr[h] = A::best(thr[h], __shfl_xor_sync(0xffffffffu, thr[h], 1));
+        thr[h] = A::best(thr[h], __shfl_xor_sync(0xffffffffu, thr[h], 2));
+        T gbest[4];
 #pragma unroll
         for (int k = 0; k < 4; k++) {                         // 8 columns of row r0 + 8h: c = 4k .. 4k + 3, e = 0, 1
-            gmax[k] = d[16 * k + 2 * h];
+            gbest[k] = d[16 * k + 2 * h];
 #pragma unroll
             for (int c = 0; c < 4; c++)
 #pragma unroll
-                for (int e = 0; e < 2; e++) gmax[k] = max(gmax[k], d[16 * k + 4 * c + 2 * h + e]);
+                for (int e = 0; e < 2; e++) gbest[k] = A::best(gbest[k], d[16 * k + 4 * c + 2 * h + e]);
         }
-        if (max(max(gmax[0], gmax[1]), max(gmax[2], gmax[3])) <= thr[h]) continue;
+        if (!A::beats(A::best(A::best(gbest[0], gbest[1]), A::best(gbest[2], gbest[3])), thr[h])) continue;
 #pragma unroll
         for (int k = 0; k < 4; k++) {
-            if (gmax[k] > thr[h]) {
+            if (A::beats(gbest[k], thr[h])) {
 #pragma unroll
                 for (int c = 0; c < 4; c++) {
 #pragma unroll
@@ -267,7 +324,7 @@ __device__ __forceinline__ void top2_rows(const typename A::T (&d)[64], int n0, 
                         k1[h] = min(k1[h], hi);
                     }
                 }
-                thr[h] = max(thr[h], A::dot_of_key(k1[h]));
+                thr[h] = A::best(thr[h], A::bound_of_key(k1[h]));
             }
         }
     }
@@ -280,7 +337,7 @@ __device__ __forceinline__ void top2_tile(typename A::T (&d)[64], int col0, int 
     const int n0 = col0 + 2 * quad;
     if (col0 + TN > nt) {                                     // only the last train tile: columns past nt hold zero rows
 #pragma unroll
-        for (int i = 0; i < 64; i++) if (n0 + 8 * (i >> 2) + (i & 1) >= nt) d[i] = A::neg();   // never opens a group
+        for (int i = 0; i < 64; i++) if (n0 + 8 * (i >> 2) + (i & 1) >= nt) d[i] = A::worst();   // never opens a group
         top2_rows<A, true>(d, n0, nt, k0, k1, thr);
     } else {
         top2_rows<A, false>(d, n0, nt, k0, k1, thr);
@@ -294,6 +351,7 @@ knn2_mma_kernel(const uint8_t* __restrict__ Aexp, const uint8_t* __restrict__ Be
                 uint2* __restrict__ partial, const MmaLayout L, int32_t* __restrict__ dbg) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* sm = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    constexpr int BLOB = blob_bytes(KIND);
     uint8_t* sA = sm;
     uint8_t* sB = sm + 2 * BLOB;
     SmemBars& B = *reinterpret_cast<SmemBars*>(sm + (2 + NSTAGE) * BLOB);
@@ -340,7 +398,7 @@ knn2_mma_kernel(const uint8_t* __restrict__ Aexp, const uint8_t* __restrict__ Be
     const int trow = (g & 1) * WM + (warp & 3) * 16 + (lane >> 2);   // row inside the A tile of accumulator row r0; r1 = r0 + 8
     const uint32_t a0 = smem_u32(sA) + (uint32_t)t * BLOB + (uint32_t)(g & 1) * L.moff;
     uint32_t k0[2] = {NONE, NONE}, k1[2] = {NONE, NONE};   // per row r0, r0 + 8: the two smallest keys (top2_tile)
-    T thr[2] = {A::neg(), A::neg()};
+    T thr[2] = {A::worst(), A::worst()};
     T d[64];
 #pragma unroll
     for (int i = 0; i < 64; i++) d[i] = T(0);
@@ -352,7 +410,7 @@ knn2_mma_kernel(const uint8_t* __restrict__ Aexp, const uint8_t* __restrict__ Be
         const uint32_t b0 = smem_u32(sB + s * BLOB);
         wg_fence();
 #pragma unroll
-        for (int j = 0; j < 8; j++) A::mma(d, make_desc(a0 + L.koff[j], L), make_desc(b0 + L.koff[j], L), j > 0 ? 1u : 0u);
+        for (int j = 0; j < A::KSTEPS; j++) A::mma(d, make_desc(a0 + L.koff[j], L), make_desc(b0 + L.koff[j], L), j > 0 ? 1u : 0u);
         wg_commit();
         wg_wait_all();
         // the accumulators are in registers: hand the stage back to the producer before the selection work
@@ -384,8 +442,12 @@ knn2_mma_kernel(const uint8_t* __restrict__ Aexp, const uint8_t* __restrict__ Be
 
 // ---------------------------------------------------------------------------------------------- host side
 int alva_g_knn_mma = 1;        // alva_set_option("knn_mma", 0 never | 1 automatic (large query sets) | 2 always)
-int alva_g_knn_mma_kind = 0;   // alva_set_option("knn_mma_kind", 0 int8 operands / int32 accumulators | 1 E4M3 operands / fp32 accumulators)
-int alva_g_knn_mma_mode = 0;   // alva_set_option("knn_mma_mode", 0 no swizzle | 1 128-byte swizzle | 2 debugging variant of 0)
+// alva_set_option("knn_mma_kind", 0 int8 operands / int32 accumulators | 1 E4M3 operands / fp32 accumulators
+//                                | 2 1-bit operands / int32 accumulators)
+int alva_g_knn_mma_kind = 2;
+// alva_set_option("knn_mma_mode", 0 no swizzle | 1 128-byte swizzle | 2 debugging variant of 0).  Kinds 0 and 1 only: the
+// 64-byte rows of kind 2 do not fill a 128-byte swizzle atom, so kind 2 always uses the unswizzled layout
+int alva_g_knn_mma_mode = 0;
 
 int alva_knn2_merge_launch(alva_ctx* ctx, const uint2* partial, int nq, int nchunks, int32_t* out, const int32_t* counts, int qcap);
 
@@ -407,6 +469,19 @@ static MmaLayout make_layout(int mode) {
         L.moff = WM * 128;
     }
     return L;
+}
+
+struct MmaArgs {
+    const uint8_t* Aexp; const uint8_t* Bexp; const int32_t* rowmap; const int32_t* total_ptr;
+    int nq, nt, b_tiles, tiles_per_chunk, nchunks; uint2* partial; int32_t* dbg;
+};
+template <int KIND>
+static int launch_mma(alva_ctx* ctx, dim3 grid, const MmaArgs& a, const MmaLayout& L) {
+    const size_t smem = (size_t)(2 + NSTAGE) * blob_bytes(KIND) + sizeof(SmemBars) + 1024;
+    ALVA_CUDA(cudaFuncSetAttribute(knn2_mma_kernel<KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    knn2_mma_kernel<KIND><<<grid, NTHREADS, smem, ctx->stream>>>(a.Aexp, a.Bexp, a.rowmap, a.total_ptr, a.nq, a.nt, a.b_tiles,
+                                                                 a.tiles_per_chunk, a.nchunks, a.partial, L, a.dbg);
+    return 0;
 }
 
 // true if the tensor-core path should serve this problem.  Measured on H100 (CUDA events, both paths on the same inputs): the
@@ -433,9 +508,10 @@ int alva_knn2_mma_launch(alva_ctx* ctx, const uint8_t* q, int nq, const uint8_t*
     nchunks = (b_tiles + tiles_per_chunk - 1) / tiles_per_chunk;
 
     // workspace: offsets | rowmap | A tiles | B tiles | dbg
+    const int kind = alva_g_knn_mma_kind;
     const size_t off_bytes = (((size_t)(counts ? nbatch + 1 : 1) * 4) + 255) & ~(size_t)255;
     const size_t map_bytes = (((size_t)a_tiles * TM * 4) + 255) & ~(size_t)255;
-    const size_t a_bytes = (size_t)a_tiles * BLOB, b_bytes = (size_t)b_tiles * BLOB;
+    const size_t a_bytes = (size_t)a_tiles * blob_bytes(kind), b_bytes = (size_t)b_tiles * blob_bytes(kind);
     const size_t need = off_bytes + map_bytes + a_bytes + b_bytes;
     if (need > ctx->knn_ws_bytes) {
         ctx->ws_epoch++;
@@ -451,32 +527,28 @@ int alva_knn2_mma_launch(alva_ctx* ctx, const uint8_t* q, int nq, const uint8_t*
     uint2* partial = (uint2*)alva_scratch(ctx, (size_t)nq * nchunks * sizeof(uint2));
     if (!partial) return ALVA_E_CUDA;
 
-    const MmaLayout L = make_layout(alva_g_knn_mma_mode);
+    const MmaLayout L = make_layout(kind == 2 ? 0 : alva_g_knn_mma_mode);
     if (counts) {
         knn2_offsets_kernel<<<1, 256, 0, ctx->stream>>>(counts, nbatch, qcap, offsets);
         ALVA_LAUNCH_CHECK(ctx);
     }
-    const int a_blocks = a_tiles * 8, b_blocks = b_tiles * 8;
-    const int kind = alva_g_knn_mma_kind ? 1 : 0;
+    const int blocks_per_tile = TM * (row_bytes(kind) / 16) / 256;   // one thread per 16-byte chunk
+    const int a_blocks = a_tiles * blocks_per_tile, b_blocks = b_tiles * blocks_per_tile;
     knn2_expand_kernel<<<a_blocks + b_blocks, 256, 0, ctx->stream>>>(q, offsets, nbatch, qcap, nq, Aexp, rowmap, a_blocks, t, nt, Bexp, L.mode, kind);
     ALVA_LAUNCH_CHECK(ctx);
 
-    const size_t smem = (size_t)(2 + NSTAGE) * BLOB + sizeof(SmemBars) + 1024;
     const dim3 grid(npairs, nchunks);
     const int32_t* total_ptr = counts ? offsets + nbatch : nullptr;
-    if (kind) {
-        ALVA_CUDA(cudaFuncSetAttribute(knn2_mma_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        knn2_mma_kernel<1><<<grid, NTHREADS, smem, ctx->stream>>>(Aexp, Bexp, rowmap, total_ptr, nq, nt, b_tiles, tiles_per_chunk, nchunks, partial, L, dbg_out);
-    } else {
-        ALVA_CUDA(cudaFuncSetAttribute(knn2_mma_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        knn2_mma_kernel<0><<<grid, NTHREADS, smem, ctx->stream>>>(Aexp, Bexp, rowmap, total_ptr, nq, nt, b_tiles, tiles_per_chunk, nchunks, partial, L, dbg_out);
-    }
+    const MmaArgs args{Aexp, Bexp, rowmap, total_ptr, nq, nt, b_tiles, tiles_per_chunk, nchunks, partial, dbg_out};
+    const int rc = kind == 2 ? launch_mma<2>(ctx, grid, args, L) : kind == 1 ? launch_mma<1>(ctx, grid, args, L)
+                                                                             : launch_mma<0>(ctx, grid, args, L);
+    if (rc) return rc;
     ALVA_LAUNCH_CHECK(ctx);
     return alva_knn2_merge_launch(ctx, partial, nq, nchunks, out, counts, qcap);
 }
 
-// Debugging aid (tools/gpu_knn_mma_check.py): run the tensor-core path unconditionally and also return the raw dot
-// products of the first 128 x 128 tile (dbg_dev: 16384 int32, device memory).
+// Debugging aid (tools/gpu_knn_mma_check.py): run the tensor-core path unconditionally and also return the raw accumulators
+// (distances for kind 2, dot products otherwise) of the first 128 x 128 tile (dbg_dev: 16384 int32, device memory).
 extern "C" int alva_debug_knn2_mma(alva_ctx* ctx, const uint8_t* q, int nq, const uint8_t* t, int nt, int32_t* out, int32_t* dbg_dev) { AlvaDeviceGuard guard__(ctx);
     if (!ctx || !q || !t || !out || nq < 1 || nt < 1 || nt >= (1 << 22)) { alva_set_error("alva_debug_knn2_mma: bad argument"); return ALVA_E_INVALID; }
     return alva_knn2_mma_launch(ctx, q, nq, t, nt, out, nullptr, 0, 0, dbg_dev);

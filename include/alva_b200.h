@@ -433,17 +433,19 @@ int alva_k_ba_local(alva_ctx*, int nprob, int nkf, int nlm, int nobs, const doub
  * 4: 80 registers / 24 warps per SM).  Results are identical.
  * "knn_mma" = 0 | 1 | 2: the tensor-core formulation of the Hamming matcher (hamming_mma.cu: descriptors expanded to +-1
  * int8, wgmma s8 x s8 -> s32, dot = 256 - 2 * distance): 0 never, 1 for large query sets (default), 2 always.  Results
- * are identical.  "knn_mma_kind" = 0 | 1: operand kind of that kernel (0: +-1 as int8, int32 accumulators -- default;
- * 1: +-1.0 as E4M3, fp32 accumulators).  "knn_mma_mode" = 0 | 1 | 2: its
- * shared-memory operand layout (0 no swizzle, 1 128-byte swizzle, 2 a debugging variant of 0 for the wgmma descriptor
- * convention, whose results are not guaranteed).
+ * are identical.  "knn_mma_kind" = 0 | 1 | 2: operand kind of that kernel (2: 1-bit rows [a | ~a] x [~b | b], wgmma
+ * .b1.and.popc, the int32 accumulator is the distance -- default; 0: +-1 as int8, int32 accumulators; 1: +-1.0 as E4M3, fp32
+ * accumulators).  "knn_mma_mode" = 0 | 1 | 2: the shared-memory operand layout of kinds 0 and 1 (0 no swizzle, 1 128-byte
+ * swizzle, 2 a debugging variant of 0 for the wgmma descriptor convention, whose results are not guaranteed); kind 2 always
+ * uses the unswizzled layout.
  * "frontend_variant" = 2 | 0: the fused front-end kernel (2: frontend_tile_kernel_v2, default; 0: the round-1 kernel, which
  * also serves geometries a TMA tensor map cannot express).  Results are identical.
  * "frontend_prefetch" = 0 | 1: variant 2 also pulls the tile at the same position a few frames ahead into L2 (TMA prefetch)
  * while it works on its own (default 0).  Results are identical. */
 int alva_set_option(const char* name, int value);
 /* Debugging aid: the tensor-core matcher unconditionally on q [nq][32] x t [nt][32] (device pointers, 16-byte aligned);
- * dbg_dev (optional, 16384 int32 of device memory) receives the raw dot products of the first 128 x 128 tile. */
+ * dbg_dev (optional, 16384 int32 of device memory) receives the raw accumulators of the first 128 x 128 tile: Hamming
+ * distances under "knn_mma_kind" 2, dot products 256 - 2 * distance under kinds 0 and 1. */
 int alva_debug_knn2_mma(alva_ctx*, const uint8_t* q, int nq, const uint8_t* t, int nt, int32_t* out, int32_t* dbg_dev);
 
 /* Residual / Jacobian build alone (DirectSE3::ReprojectionErrorKSE3AnchInvDepth::Evaluate,

@@ -85,7 +85,8 @@ def per_launch(n=10):
     return res
 
 
-configs = [dict(knn_mma_mode=mode, knn_mma_kind=kind) for mode in (0, 1) for kind in (0, 1)]
+# kind 2 (1-bit operands) has one layout: knn_mma_mode does not apply to it
+configs = [dict(knn_mma_mode=mode, knn_mma_kind=kind) for mode in (0, 1) for kind in (0, 1)] + [dict(knn_mma_mode=0, knn_mma_kind=2)]
 result = {"card": card(), "problem": f"{nb} x {qcap} slots, {live} live, {nt} map rows", "macs": macs,
           "int8_tensor_floor_us_at_1979_tops": round(2 * macs / 1979e12 * 1e6, 1), "configs": [], "per_launch": []}
 print(result["card"], flush=True)
@@ -102,12 +103,12 @@ for cfg in configs:
                same_output=bool(np.array_equal(got, ref)))
     print(row, flush=True)
     result["configs"].append(row)
-for mode in (0, 1):
+for mode, kind in ((0, 0), (1, 0), (0, 2)):
     assert L.alva_set_option(b"knn_mma_mode", mode) == 0
-    assert L.alva_set_option(b"knn_mma_kind", 0) == 0
-    result["per_launch"].append({"knn_mma_mode": mode, "knn_mma_kind": 0, "kernels": per_launch()})
+    assert L.alva_set_option(b"knn_mma_kind", kind) == 0
+    result["per_launch"].append({"knn_mma_mode": mode, "knn_mma_kind": kind, "kernels": per_launch()})
     print(result["per_launch"][-1], flush=True)
-for k, v in (("knn_mma", 1), ("knn_mma_mode", 0), ("knn_mma_kind", 0)):
+for k, v in (("knn_mma", 1), ("knn_mma_mode", 0), ("knn_mma_kind", 2)):
     L.alva_set_option(k.encode(), v)
 if args.out:
     with open(args.out, "w") as f:

@@ -1,6 +1,7 @@
-"""GPU check of the tensor-core Hamming matcher (hamming_mma.cu): raw dot products of the first tile and the final
-2-NN lists against numpy, for one shared-memory layout mode (argv[1]), then timing against the LOP3/POPC kernel on the
-bench's shape.  Run one mode per process (a bad descriptor traps the context):  python tools/gpu_knn_mma_check.py 0"""
+"""GPU check of the tensor-core Hamming matcher (hamming_mma.cu): raw accumulators of the first tile (dot products for
+operand kinds 0 and 1, distances for kind 2) and the final 2-NN lists against numpy, for one shared-memory layout mode
+(argv[1]) and operand kind (argv[3]), then timing against the LOP3/POPC kernel on the bench's shape.  Run one mode per
+process (a bad descriptor traps the context):  python tools/gpu_knn_mma_check.py 0 time 2"""
 import ctypes as C
 import os
 import sys
@@ -59,7 +60,7 @@ for (nq, nt) in [(128, 128), (300, 1000), (1000, 2500), (257, 129)]:
         sys.exit(2)
     g = dbg.cpu().numpy()
     m, n = min(nq, 128), min(nt, 128)
-    want = 256 - 2 * ham(q[:m], t[:n])
+    want = ham(q[:m], t[:n]) if kind == 2 else 256 - 2 * ham(q[:m], t[:n])
     tile_ok = np.array_equal(g[:m, :n], want)
     got = out.cpu().numpy()
     ref = ref_knn2(q, t)
